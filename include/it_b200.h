@@ -165,7 +165,9 @@ int it_b200_batchnorm_relu(int dtype, const void *x, const float *mean, const fl
 int64_t it_b200_matmul_workspace(int dtype, int64_t b, int m, int n, int k);
 /* Kernel selection for this thread's following it_b200_matmul calls -- what MatMul's tune() records per shape in PerfEngine and its
  * compute(op, record) re-applies (reference: the cuBLAS algorithm index of MatmulCublasPerfRecordObj, matmul.cc:12-24,187-208).
- * impl: 0 production dispatch, 1 gemm_skinny (mma.sync + cluster split-K), 2 gemm_tc (wgmma), 3 gemm_simt; skinny_nb: 0 auto, 1, 2. */
+ * impl: 0 production dispatch, 1 gemm_skinny (mma.sync + cluster split-K), 2 gemm_tc (wgmma), 3 gemm_simt; skinny_nb: 0 auto, 1, 2.
+ * A pinned kernel that does not take a shape falls through to gemm_simt.  Also honoured by it_b200_matmul_grouped (only the pinned
+ * kernel's grouped launch) and it_b200_matmul_fused (returns 2 unless impl is 0 or 2). */
 void it_b200_matmul_select(int impl, int skinny_nb);
 int it_b200_matmul(int dtype, const void *A, const void *B, const void *bias, void *C, int64_t b,
                    int m, int n, int k, int64_t stride_a, int64_t stride_b, int trans_a,
@@ -261,13 +263,6 @@ int it_b200_conv2d_nhwc(int dtype, const void *x, const void *w, void *y, int y_
                         int S, int ph, int pw, int sh, int sw, int dh, int dw, const float *bn_mean, const float *bn_var,
                         const float *bn_scale, const float *bn_bias, float bn_eps, const void *residual, int relu,
                         void *workspace, int64_t workspace_bytes, void *stream);
-
-/* L2 prefetch hint (optional, per host thread): [ptr, ptr + bytes) is constant data (weights) that the kernel AFTER the next launch
- * will stream.  The next it_b200_attention_kvcache* launch spreads `cp.async.bulk.prefetch.L2` over its own run time -- the decode
- * attention kernel uses ~70 % of HBM, the following projection's weights ride the rest and are then read from L2 -- and clears the
- * hint.  Launchers that do not use it ignore it.  The attention kernel can lose more to the extra traffic than the projection
- * gains, so the hint is honoured only under ITB_L2_PREFETCH=1. */
-void it_b200_l2_prefetch_hint(const void *ptr, long long bytes);
 
 /* ---- AttentionKVCache (decode, q-len 1): replaces _attention_kvcache_kernel_128_1/_2
  *      (attention_kvcache.cu:8-169).  Appends k,v IN PLACE into k_cache/v_cache at

@@ -55,7 +55,6 @@ _SIGS = {
     "it_b200_pool2d": (c_int, [c_int, c_int, vp, vp] + [c_int] * 14 + [vp]),
     "it_b200_pool2d_nhwc": (c_int, [c_int, c_int, vp, vp] + [c_int] * 14 + [vp]),
     "it_b200_batchnorm": (c_int, [c_int, vp, vp, vp, vp, vp, vp, c_int, c_int, c_int64, c_float, vp]),
-    "it_b200_l2_prefetch_hint": (None, [vp, ctypes.c_longlong]),
     "it_b200_matmul_select": (None, [c_int, c_int]),
     "it_b200_matmul_workspace": (c_int64, [c_int, c_int64, c_int, c_int, c_int]),
     "it_b200_matmul": (c_int, [c_int, vp, vp, vp, vp, c_int64, c_int, c_int, c_int, c_int64, c_int64, c_int, c_int,

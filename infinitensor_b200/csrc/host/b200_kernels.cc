@@ -521,12 +521,7 @@ void runAttentionRope(const Operator &ropeQ, const Operator &ropeK, const Operat
                                       P(att->getOutput()), d[0], d[1], d[2], d[3], ws, wsb, S()), att);
 }
 
-bool runPrefillAttention(const OpVec &ops, const RuntimeObj *) {
-    static const bool off = [] {
-        const char *e = std::getenv("ITB_NO_PREFILL_ATTENTION");
-        return e && e[0] == '1';
-    }();
-    if (off) return false;
+void runPrefillAttention(const OpVec &ops, const RuntimeObj *) {
     // extended form (schedule.cc extendPrefillChain): {Split, Rq, Tq, Rk, Tk, Rv, Tv, <chain>, mm2, Tout, Rout}
     const bool ext = ops[0]->getOpType() == OpType::Split;
     const size_t c0 = ext ? 7 : 0, cend = ext ? ops.size() - 2 : ops.size();  // [c0, cend) = Transpose(k), mm1, .., Softmax, mm2
@@ -561,21 +556,15 @@ bool runPrefillAttention(const OpVec &ops, const RuntimeObj *) {
         const int64_t es = (int64_t)qkv->getDType().getSize();
         CK(it_b200_attention_prefill_strided(DTI(q), base, base + d * es, base + 2 * d * es, P(fin), (int)B, (int)H, (int)Sq, (int)k->getDims()[2],
                                              (int)D, view, view, view, ost, scale, isDiv, maskp, ms[0], ms[1], ms[2], ms[3], S()), mm2);
-        return true;
+        return;
     }
     CK(it_b200_attention_prefill(DTI(q), P(q), P(k), P(v), P(out), qd[0], qd[1], qd[2], k->getDims()[2], qd[3], scale, isDiv, maskp,
                                  ms[0], ms[1], ms[2], ms[3], S()), mm2);
-    return true;
 }
 
 // DecoderStack: st.sub = per layer { RMSNorm | MatMulGroup{3} | AttentionRope | MatMulAdd | RMSNorm | MatMulGroup{2} | SiluMul |
 // MatMulAdd } with Alias steps in between (schedule.cc: matchDecoderLayer)
 bool runDecoderStack(const ExecStep &st, const RuntimeObj *ctx) {
-    static const bool off = [] {
-        const char *e = std::getenv("ITB_NO_DECODE_STACK");
-        return e && e[0] == '1';
-    }();
-    if (off) return false;
     vector<const ExecStep *> cs;
     for (auto &sb : st.sub) {
         if (sb.kind == ExecStep::Alias) {
@@ -724,22 +713,6 @@ bool runConvBnAct(const OpVec &ops, const RuntimeObj *ctx, int layout) {
     if (rc == 2) return false;
     CK(rc, ops.back());
     return true;
-}
-
-// Step i is a decode attention launch: tell it which weights the next GEMM will stream (it_b200_l2_prefetch_hint) -- the attention
-// kernel leaves ~30 % of HBM idle and the next GEMM cannot become resident beside it, so its weights are prefetched into L2 meanwhile
-void setPrefetchHint(const vector<ExecStep> &sched, size_t i) {
-    const auto &st = sched[i];
-    if (st.ops.back()->getOpType() != OpType::AttentionKVCache) return;
-    for (size_t j = i + 1; j < sched.size() && j <= i + 6; ++j) {
-        const auto &nx = sched[j];
-        if (nx.kind == ExecStep::Alias) continue;
-        if (nx.ops[0]->getOpType() != OpType::MatMul) return;
-        auto w = nx.ops[0]->getInputs(1);
-        if (!w->isWeight() || w->getBytes() > (size_t)24 << 20) return;  // (leave room in the 50 MB L2 for the stream itself)
-        it_b200_l2_prefetch_hint(P(w), (long long)w->getBytes());
-        return;
-    }
 }
 
 // every NHWC conv of the schedule with filters larger than 1x1: re-order all the filter banks in one launch, into buffers the

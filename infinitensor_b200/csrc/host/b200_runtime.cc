@@ -208,7 +208,6 @@ void CudaRuntimeObj::runWithoutSyncImpl(const Graph &graph, bool validate) const
                 if (on) nvtxRangePop();
             }
         } range(nvtx, st);
-        b200::setPrefetchHint(sched, i);
         execStep(st, plan[i].kernel, plan[i].record ? &*plan[i].record : nullptr);
         cudaError_t err = cudaPeekAtLastError();
         if (err != cudaSuccess) {
@@ -261,10 +260,7 @@ void CudaRuntimeObj::execStep(const ExecStep &st, Kernel *kernel, const PerfReco
             // no NVLink peer comm (or shape outside its limits): the ordinary kernels, one by one
             for (auto &m : st.ops) reg.getKernel(KernelAttrs{Device::CUDA, m->getOpType().underlying()})->compute(m, this);
         break;
-    case ExecStep::PrefillAttention:
-        if (!b200::runPrefillAttention(st.ops, this))
-            for (auto &m : st.ops) reg.getKernel(KernelAttrs{Device::CUDA, m->getOpType().underlying()})->compute(m, this);
-        break;
+    case ExecStep::PrefillAttention: b200::runPrefillAttention(st.ops, this); break;
     case ExecStep::DecoderStack:
         if (!b200::runDecoderStack(st, this))
             for (auto &sb : st.sub) execStep(sb, nullptr, nullptr);

@@ -164,11 +164,10 @@ bool matmulAddIsPlain(const OpVec &ops);  // {bias-free MatMul, Add}: the residu
 bool runMatmulFused(const OpVec &ops, const RuntimeObj *ctx);
 bool runConvBnAct(const OpVec &ops, const RuntimeObj *ctx, int layout = 0);
 void prepConvFilters(const vector<ExecStep> &sched, const RuntimeObj *ctx);
-void setPrefetchHint(const vector<ExecStep> &sched, size_t i);
 void runPoolNhwc(const Operator &op, const RuntimeObj *ctx);
 void runAttentionRope(const Operator &ropeQ, const Operator &ropeK, const Operator &att, const RuntimeObj *ctx);
-// {Transpose(k), MatMul, [Div | Mul], [Add], Softmax, MatMul} as one fused wgmma attention kernel; false = not taken
-bool runPrefillAttention(const OpVec &ops, const RuntimeObj *ctx);
+// {Transpose(k), MatMul, [Div | Mul], [Add], Softmax, MatMul} as one fused wgmma attention kernel
+void runPrefillAttention(const OpVec &ops, const RuntimeObj *ctx);
 // L decoder layers through the persistent kernel; false = not taken (nothing launched): run `st.sub` step by step
 bool runDecoderStack(const ExecStep &st, const RuntimeObj *ctx);
 }  // namespace b200

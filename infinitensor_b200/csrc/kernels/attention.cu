@@ -16,7 +16,6 @@
 // 32 for fp32), U independent K and V loads are issued before any arithmetic so each lane keeps
 // 2*U 16-byte requests in flight.
 #include <algorithm>
-#include <cstdlib>
 #include <string>
 
 #include "common.cuh"
@@ -37,17 +36,18 @@ template <typename P> __device__ __forceinline__ int read_pos(const void *p, int
 // ------------------------------------------------------------------------------------------------------------------
 // attn_stream_kernel: the production decode kernel.  Same arithmetic per cache row as attn_decode_kernel, but
 //   * the (head, 64-row chunk) work units of the whole batch are FLATTENED and dealt out in equal contiguous ranges to
-//     a persistent grid of `ctas_per_sm x 132` CTAs -- B*H = 512 heads over 296 CTA slots no longer costs a 1.73-wave
-//     tail (the split-per-head grid ran at 86 % occupancy of its last wave);
+//     a persistent grid of 2 x 132 CTAs -- a head count that is not a multiple of the CTA slots no longer costs a
+//     partly filled last wave, as a split-per-head grid does;
 //   * every chunk of K rows and of V rows is ONE contiguous 16 KiB range of the cache ([B,H,S,128] layout), so a
 //     producer warp streams it HBM -> shared memory with cp.async.bulk (TMA 1-D) through a full/empty mbarrier ring;
-//     bytes in flight are set by the ring depth (3 x 32 KiB per CTA), not by registers per thread;
+//     bytes in flight are set by the ring depth (2 x 32 KiB per CTA), not by registers per thread;
 //   * a head whose units straddle two or three CTAs is finished by the LAST of them to arrive (self-cleaning ticket per
 //     head), which merges the (m, l, acc) partials in CTA order -- deterministic, no second kernel.
 // The in-place append and the appended row's contribution are done by the CTA that owns the head's last chunk, from
 // registers; chunk loads stop at row pos-1, so the append never races the bulk reads.
 // ------------------------------------------------------------------------------------------------------------------
-constexpr int AS_MAX_STAGES = 6;
+constexpr int AS_STAGES = 2;  // ring depth
+constexpr int AS_CTAS_PER_SM = 2;
 
 template <typename T, int EPL, int LPR>
 __device__ __forceinline__ void rope_one(Vec16<T> &x, int col, const float *cs_t, const float *sn_t) {
@@ -73,19 +73,19 @@ __device__ __forceinline__ void rope_one(Vec16<T> &x, int col, const float *cs_t
 constexpr int AS_MAX_B = 1024;  // batch rows whose (position, chunk count) the CTA keeps in shared memory
 
 template <typename T, int WARPS, int U, bool ROPE>
-__global__ void __launch_bounds__((WARPS + 1) * 32, 2)
+__global__ void __launch_bounds__((WARPS + 1) * 32, AS_CTAS_PER_SM)
     attn_stream_kernel(T *__restrict__ kcache, T *__restrict__ vcache, const T *__restrict__ q,
                        const T *__restrict__ kin, const T *__restrict__ vin, const void *__restrict__ position_id,
                        int pos_flags, T *__restrict__ out, int Smax, int BH, float *__restrict__ partial,
                        int slots_per_head, int *__restrict__ tickets, const void *__restrict__ rope_pos,
-                       int rope_pos_dtype, int H, int stages, const unsigned char *__restrict__ pf_ptr, long long pf_bytes) {
+                       int rope_pos_dtype, int H) {
     using C = RowCfg<T>;
     constexpr int EPL = C::EPL, LPR = C::LPR, RPW = C::RPW;
     constexpr int CH = WARPS * RPW * U;                       // cache rows per chunk
     constexpr int CHUNK_BYTES = CH * kD * (int)sizeof(T);     // 16 KiB for every dtype
     constexpr int CONSUMERS = WARPS * 32;
     extern __shared__ __align__(128) unsigned char ring[];    // stages x { K chunk | V chunk }
-    __shared__ __align__(8) uint64_t full[AS_MAX_STAGES], empty[AS_MAX_STAGES];
+    __shared__ __align__(8) uint64_t full[AS_STAGES], empty[AS_STAGES];
     __shared__ float s_m[WARPS], s_l[WARPS];
     __shared__ float s_acc[WARPS][kD];
     __shared__ float s_cs[kD / 2], s_sn[kD / 2];
@@ -103,7 +103,7 @@ __global__ void __launch_bounds__((WARPS + 1) * 32, 2)
     if (pos_flags & ITB_POS_IN_STEP) pdl_wait();
     const int Bn = BH / H;
     if (threadIdx.x == 0) {
-        for (int s = 0; s < stages; ++s) {
+        for (int s = 0; s < AS_STAGES; ++s) {
             mbar_init(&full[s], 1);
             mbar_init(&empty[s], WARPS);
         }
@@ -162,19 +162,7 @@ __global__ void __launch_bounds__((WARPS + 1) * 32, 2)
         if (lane == 0) {
             const uint64_t policy = l2_policy_evict_first();
             int st = 0, ph = 0;
-            // L2 prefetch hint (it_b200_l2_prefetch_hint): this CTA's slice of the next GEMM's weights, 16 KB per unit it streams
-            long long pf_off = 0, pf_end = 0;
-            if (pf_bytes > 0) {
-                const long long per = (((pf_bytes + G - 1) / G) + 16383) & ~16383ll;
-                pf_off = (long long)blockIdx.x * per;
-                pf_end = min(pf_bytes, pf_off + per) & ~15ll;
-            }
-            const int pf_per_unit = nunits > 0 ? (int)((pf_end - pf_off + 16383) / 16384 + nunits - 1) / nunits : 0;
             for (int it = 0; it < nunits; ++it) {
-                for (int i = 0; i < pf_per_unit && pf_off < pf_end; ++i, pf_off += 16384) {
-                    const uint32_t n = (uint32_t)min(16384ll, pf_end - pf_off);
-                    asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(pf_ptr + pf_off), "r"(n) : "memory");
-                }
                 mbar_wait(&empty[st], ph ^ 1);
                 const int rows = min(CH, pos - c * CH);
                 if (rows > 0) {
@@ -187,7 +175,7 @@ __global__ void __launch_bounds__((WARPS + 1) * 32, 2)
                     mbar_arrive(&full[st]);
                 }
                 next_unit();
-                if (++st == stages) { st = 0; ph ^= 1; }
+                if (++st == AS_STAGES) { st = 0; ph ^= 1; }
             }
         }
         return;
@@ -309,7 +297,7 @@ __global__ void __launch_bounds__((WARPS + 1) * 32, 2)
 #endif
         __syncwarp();
         if (lane == 0) mbar_arrive(&empty[st]);  // this warp is done with the stage
-        if (++st == stages) { st = 0; ph ^= 1; }
+        if (++st == AS_STAGES) { st = 0; ph ^= 1; }
 
         const bool last_chunk = c == nch - 1;
         if (last_chunk && warp == 0) {
@@ -424,10 +412,6 @@ __global__ void __launch_bounds__((WARPS + 1) * 32, 2)
 
 using namespace itb;
 
-static int env_int(const char *name, int dflt) {
-    const char *e = std::getenv(name);
-    return e && *e ? std::atoi(e) : dflt;
-}
 static int stream_slots_per_head(int S_max) { return S_max / 32 + 1; }  // >= chunks per head for every dtype
 
 extern "C" int64_t it_b200_attention_kvcache_workspace(int B, int H, int S_max, int D) {
@@ -435,30 +419,23 @@ extern "C" int64_t it_b200_attention_kvcache_workspace(int B, int H, int S_max, 
     return (int64_t)B * H * stream_slots_per_head(S_max) * (kD + 2) * sizeof(float);
 }
 
-template <typename T, bool ROPE, int WARPS, int U>
-static int launch_attn_stream_cfg(T *kc, T *vc, const T *q, const T *k, const T *v, const void *position_id, int pos_flags,
+template <typename T, bool ROPE>
+static int launch_attn_stream(T *kc, T *vc, const T *q, const T *k, const T *v, const void *position_id, int pos_flags,
                               const void *rope_pos, int rope_pos_dtype, T *out, int BH, int H, int S_max,
-                              float *workspace, cudaStream_t st, const void *pf_ptr, long long pf_bytes) {
+                              float *workspace, cudaStream_t st) {
+    constexpr int WARPS = 8, U = 4;  // consumer warps x rows per lane and chunk
     constexpr int CH = WARPS * RowCfg<T>::RPW * U;
-    static const int stages = std::max(2, std::min(AS_MAX_STAGES, env_int("ITB_ATTN_STAGES", 2)));
-    static const int per_sm = std::max(1, std::min(2, env_int("ITB_ATTN_CTAS_PER_SM", 2)));
-    const size_t smem = (size_t)stages * 2 * CH * kD * sizeof(T);
+    const size_t smem = (size_t)AS_STAGES * 2 * CH * kD * sizeof(T);
     auto kern = attn_stream_kernel<T, WARPS, U, ROPE>;
     // the attribute is per DEVICE: a process may own runtimes on several GPUs
     if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) return 1;
     int *tickets = stream_tickets(st, BH);
     if (!tickets) return 1;
     const int64_t max_units = (int64_t)BH * (S_max / CH + 1);
-    const int grid = (int)std::min<int64_t>(max_units, (int64_t)per_sm * kNumSMs);
+    const int grid = (int)std::min<int64_t>(max_units, (int64_t)AS_CTAS_PER_SM * kNumSMs);
     cudaError_t e = launch_k(kern, dim3(grid), dim3((WARPS + 1) * 32), smem, st, kc, vc, q, k, v, position_id, pos_flags,
-                             out, S_max, BH, workspace, stream_slots_per_head(S_max), tickets, rope_pos, rope_pos_dtype,
-                             H, stages, (const unsigned char *)pf_ptr, pf_bytes);
+                             out, S_max, BH, workspace, stream_slots_per_head(S_max), tickets, rope_pos, rope_pos_dtype, H);
     return e == cudaSuccess ? 0 : 1;
-}
-// consumer warps x rows per lane and chunk: 8 x 4 (default, measured best) or 16 x 2 (ITB_ATTN_WARPS=16)
-template <typename T, bool ROPE, typename... A> static int launch_attn_stream(A... a) {
-    static const int warps = env_int("ITB_ATTN_WARPS", 8);
-    return warps == 8 ? launch_attn_stream_cfg<T, ROPE, 8, 4>(a...) : launch_attn_stream_cfg<T, ROPE, 16, 2>(a...);
 }
 
 static int attention_impl(int dtype, void *k_cache, void *v_cache, const void *q, const void *k, const void *v,
@@ -480,17 +457,13 @@ static int attention_impl(int dtype, void *k_cache, void *v_cache, const void *q
     ITB_CHECK(workspace && workspace_bytes >= need, "AttentionKVCache: workspace %lld < %lld bytes",
               (long long)workspace_bytes, (long long)need);
     auto st = (cudaStream_t)stream;
-    const void *pf_ptr = nullptr;
-    long long pf_bytes = 0;
-    take_prefetch_hint(pf_ptr, pf_bytes);
-    if (!aligned16(pf_ptr)) pf_bytes = 0;
     ITB_DISPATCH_FLOAT(dtype, "AttentionKVCache", {
         int rc = rope_pos ? launch_attn_stream<T, true>((T *)k_cache, (T *)v_cache, (const T *)q, (const T *)k,
                                                         (const T *)v, position_id, pos_flags, rope_pos,
-                                                        rope_pos_dtype, (T *)out, BH, H, S_max, (float *)workspace, st, pf_ptr, pf_bytes)
+                                                        rope_pos_dtype, (T *)out, BH, H, S_max, (float *)workspace, st)
                           : launch_attn_stream<T, false>((T *)k_cache, (T *)v_cache, (const T *)q, (const T *)k,
                                                          (const T *)v, position_id, pos_flags, nullptr, 0, (T *)out,
-                                                         BH, H, S_max, (float *)workspace, st, pf_ptr, pf_bytes);
+                                                         BH, H, S_max, (float *)workspace, st);
         ITB_CHECK(rc == 0, "AttentionKVCache: streaming kernel launch failed: %s",
                   cudaGetErrorString(cudaGetLastError()));
         ITB_LAUNCH_CHECK("AttentionKVCache");

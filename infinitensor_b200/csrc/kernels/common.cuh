@@ -15,7 +15,6 @@ namespace itb {
 // ---- error reporting (the C spelling of infini::Exception) -------------------------------
 void set_error(const char *fmt, ...);
 void count_launch(int n = 1);
-void take_prefetch_hint(const void *&ptr, long long &bytes);  // it_b200_l2_prefetch_hint (support.cu)
 
 #define ITB_FAIL(...)                                                                          \
     do {                                                                                       \

@@ -17,8 +17,6 @@
 // Replaces cudnnConvolutionForward + the separate BatchNorm / Add / Relu kernels (reference src/kernels/cuda/conv.cc:143-168,
 // batch_norm.cc:9-69, element_wise.cu) for the ResNet-style Conv -> BN -> [Add] -> [Relu] chains.
 #include <algorithm>
-#include <cstdio>
-#include <cstdlib>
 #include <mutex>
 
 #include <cudaTypedefs.h>
@@ -49,8 +47,6 @@ struct ConvNhwcParams {
     int y_nhwc;
     int P, OW, M, F, FT, tiles_f, tiles, cchunks, Cp, RS, S, sh, sw, ph, pw, dh, dw;
     int stages, b_bytes, stg_off;
-    unsigned long long *trace;  // ITB_CONV_TRACE=1 (tools only): globaltimer stamps of CTA 0 -- [0..255] load issued, [256..511] stage
-                                // landed (MMA thread), [512..767] tile accumulator complete (epilogue), [768..1023] tile stored
 };
 
 __device__ __forceinline__ bool mbar_try_wait_addr(uint32_t bar_addr, uint32_t parity) {
@@ -63,13 +59,6 @@ __device__ __forceinline__ bool mbar_try_wait_addr(uint32_t bar_addr, uint32_t p
         : "r"(bar_addr), "r"(parity)
         : "memory");
     return ok != 0;
-}
-__device__ __forceinline__ void cv_stamp(unsigned long long *trace, int slot) {
-    if (trace && blockIdx.x == 0) {
-        unsigned long long t;
-        asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
-        trace[slot] = t;
-    }
 }
 __device__ __forceinline__ void tma_store_2d(const CUtensorMap *m, const void *smem_src, int c0, int c1) {
     asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];" ::"l"(reinterpret_cast<uint64_t>(m)),
@@ -299,7 +288,6 @@ __global__ void __launch_bounds__(CV_THREADS, 1) conv_nhwc_kernel(const __grid_c
                 cur_ft = ft;
             }
             mbar_wait(acc_full, it & 1);
-            if (threadIdx.x == 0 && it < 256) cv_stamp(p.trace, 512 + it);
             const int64_t gm = (int64_t)mt * CV_BM + row;
             const bool ok = gm < p.M;
             if (p.y_nhwc) {
@@ -381,7 +369,6 @@ __global__ void __launch_bounds__(CV_THREADS, 1) conv_nhwc_kernel(const __grid_c
             }
             __syncwarp();
             if (lane == 0) mbar_arrive(acc_empty);
-            if (threadIdx.x == 0 && it < 256) cv_stamp(p.trace, 768 + it);
         }
         if (lane == 0) bulk_wait_all();  // every TMA store of this warp is complete before the CTA (and its shared memory) goes away
     }
@@ -532,13 +519,6 @@ static int launch_conv_nhwc_t(bool is_bf16, const void *x, const void *wk, int C
     const int fixed = stg_bytes + p.FT * ACC_LD * 4 + p.FT * 8 + (16 * 2 + 2 + CV_EPI_WARPS * CV_RING) * 8 + 64 + 1024;
     // bytes in flight, not stage count, is what hides the L2 latency: 3 x 48 KB is as good as 4 (measured bound: L2 -> SM bandwidth)
     p.stages = std::max(2, std::min(6, (225 * 1024 - fixed) / stage_bytes));
-    {
-        static const int st_env = [] {
-            const char *e = std::getenv("ITB_CONV_STAGES");
-            return e && e[0] ? std::atoi(e) : 0;
-        }();
-        if (st_env >= 2 && st_env <= p.stages) p.stages = st_env;
-    }
     p.stg_off = p.stages * stage_bytes;
     const int smem = p.stages * stage_bytes + fixed;
 
@@ -579,36 +559,9 @@ static int launch_conv_nhwc_t(bool is_bf16, const void *x, const void *wk, int C
             attr_smem[dev] = smem;
         }
     }
-    static const bool tracing = [] {
-        const char *e = std::getenv("ITB_CONV_TRACE");
-        return e && e[0] == '1';
-    }();
-    static unsigned long long *trace_dev = nullptr;
-    if (tracing) {
-        if (!trace_dev) cudaMalloc(&trace_dev, 1024 * sizeof(unsigned long long));
-        cudaMemsetAsync(trace_dev, 0, 1024 * sizeof(unsigned long long), st);
-        p.trace = trace_dev;
-    }
     cudaError_t e = launch_k(kern, dim3(std::min(p.tiles, kNumSMs)), dim3(CV_THREADS), (size_t)smem, st, mapA, mapB, mapY, mapR, p);
     ITB_CHECK(e == cudaSuccess, "conv(nhwc): launch failed: %s", cudaGetErrorString(e));
     count_launch();
-    if (tracing) {  // tools/conv_bench.py with CONV_BENCH_REPS=1: one line per launch
-        static unsigned long long h[1024];
-        cudaStreamSynchronize(st);
-        cudaMemcpy(h, trace_dev, sizeof(h), cudaMemcpyDeviceToHost);
-        const unsigned long long t0 = h[0];
-        fprintf(stderr, "conv trace C=%d F=%d %dx%d M=%d FT=%d stages=%d ktiles/tile=%d tiles=%d\n", C, F, R, S, p.M, p.FT, p.stages,
-                p.RS * p.cchunks, p.tiles);
-        fprintf(stderr, "  issue :");
-        for (int i = 0; i < 40 && h[i]; ++i) fprintf(stderr, " %.2f", (double)(h[i] - t0) / 1e3);
-        fprintf(stderr, "\n  landed:");
-        for (int i = 0; i < 40 && h[256 + i]; ++i) fprintf(stderr, " %.2f", (double)(h[256 + i] - t0) / 1e3);
-        fprintf(stderr, "\n  acc   :");
-        for (int i = 0; i < 12 && h[512 + i]; ++i) fprintf(stderr, " %.2f", (double)(h[512 + i] - t0) / 1e3);
-        fprintf(stderr, "\n  stored:");
-        for (int i = 0; i < 12 && h[768 + i]; ++i) fprintf(stderr, " %.2f", (double)(h[768 + i] - t0) / 1e3);
-        fprintf(stderr, "\n");
-    }
     return 0;
 }
 

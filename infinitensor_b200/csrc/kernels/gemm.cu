@@ -8,8 +8,6 @@
 // (the "conv/im2col-GEMM path" BASELINE.json names for ResNet-50).
 #include <cudaTypedefs.h>
 
-#include <cstdlib>
-#include <cstring>
 #include <mutex>
 
 #include "conv_shapes.h"
@@ -167,26 +165,22 @@ __global__ void __launch_bounds__(256) pad_rows_kernel(const T *__restrict__ w, 
     }
 }
 
-// Kernel selection.  ITB_GEMM_IMPL = tc | skinny | simt pins one implementation (A/B testing and the parity
-// tests that must exercise each kernel); unset = the production order below.
-// per-thread kernel selection for the NEXT it_b200_matmul call(s) (it_b200_matmul_select: MatMul's tune() and tuned compute())
-static thread_local int g_sel_impl = 0;
+// Kernel selection: the production order below, unless it_b200_matmul_select pinned one kernel for this thread's next calls
+// (MatMul's tune() and tuned compute(), and the parity tests that must exercise each kernel)
+enum { SEL_AUTO = 0, SEL_SKINNY = 1, SEL_TC = 2, SEL_SIMT = 3 };
+static thread_local int g_sel_impl = SEL_AUTO;
 
 static int run_gemm(int dtype, const GemmArgs &g, cudaStream_t st) {
     if (g.batch == 0 || g.m == 0 || g.n == 0) return 0;
-    const char *pin = std::getenv("ITB_GEMM_IMPL");
-    static const char *const sel_names[] = {"", "skinny", "tc", "simt"};
-    if (!(pin && pin[0]) && g_sel_impl >= 1 && g_sel_impl <= 3) pin = sel_names[g_sel_impl];
     int r = -1;
-    if (pin && pin[0]) {
-        if (!strcmp(pin, "tc")) r = launch_gemm_tc(dtype, g, st);
-        else if (!strcmp(pin, "skinny")) r = launch_gemm_skinny(dtype, g, st);
-        else if (strcmp(pin, "simt")) ITB_FAIL("matmul: unknown ITB_GEMM_IMPL '%s'", pin);
+    if (g_sel_impl != SEL_AUTO) {
+        if (g_sel_impl == SEL_TC) r = launch_gemm_tc(dtype, g, st);
+        else if (g_sel_impl == SEL_SKINNY) r = launch_gemm_skinny(dtype, g, st);
         if (r >= 0) return r;
         return launch_gemm_simt(dtype, g, st);
     }
     // decode rows with enough 128-wide column tiles to fill the SMs without split-K (logits): wgmma swap-AB
-    if (g.m <= 64 && g.batch == 1 && !g.trans_a && !g.trans_b && (g.n + 127) / 128 >= tc_min_tiles_decode()) {
+    if (g.m <= 64 && g.batch == 1 && !g.trans_a && !g.trans_b && (g.n + 127) / 128 >= TC_MIN_TILES_DECODE) {
         GemmArgs gt = g;
         gt.no_splitk = 1;
         r = launch_gemm_tc(dtype, gt, st);
@@ -206,10 +200,11 @@ using namespace itb;
 extern "C" int64_t it_b200_matmul_workspace(int, int64_t, int, int, int) { return 0; }
 
 extern "C" void it_b200_tune_skinny(int nb, int splitk);
-// impl: 0 production order, 1 gemm_skinny, 2 gemm_tc, 3 gemm_simt (a kernel that does not take the shape falls through to gemm_simt,
-// like ITB_GEMM_IMPL); skinny_nb: 1 / 2 = 64- / 128-column tiles, 0 automatic.  Stays in force on this thread until called again.
+// impl: 0 production order, 1 gemm_skinny, 2 gemm_tc, 3 gemm_simt (a kernel that does not take the shape falls through to
+// gemm_simt; it_b200_matmul_grouped / _fused skip the grouped or fused launch of a kernel that is not the pinned one);
+// skinny_nb: 1 / 2 = 64- / 128-column tiles, 0 automatic.  Stays in force on this thread until called again.
 extern "C" void it_b200_matmul_select(int impl, int skinny_nb) {
-    g_sel_impl = impl >= 0 && impl <= 3 ? impl : 0;
+    g_sel_impl = impl >= SEL_AUTO && impl <= SEL_SIMT ? impl : SEL_AUTO;
     it_b200_tune_skinny(skinny_nb, 0);
 }
 
@@ -238,8 +233,7 @@ extern "C" int it_b200_matmul_fused(int dtype, const void *A, const void *B, con
     GemmArgs g{A, B, bias, C, b, m, n, k, stride_a, stride_b, trans_a, trans_b, bias_stride_b, bias_stride_m, bias_stride_n, act};
     g.residual = residual;
     g.no_splitk = 1;
-    const char *pin = std::getenv("ITB_GEMM_IMPL");
-    if (pin && pin[0] && strcmp(pin, "tc")) return 2;
+    if (g_sel_impl != SEL_AUTO && g_sel_impl != SEL_TC) return 2;
     if (!aligned16(C) || (residual && !aligned16(residual)) || (g.act & 0xff) == 0 && !residual) return 2;
     const int r = launch_gemm_tc(dtype, g, (cudaStream_t)stream);
     return r < 0 ? 2 : r;
@@ -250,12 +244,11 @@ extern "C" int it_b200_matmul_grouped(int dtype, const void *X, int n_groups, co
     ITB_CHECK(n_groups >= 1, "matmul_grouped: no groups");
     auto st = (cudaStream_t)stream;
     GemmArgs g{X, W[0], nullptr, C[0], 1, m, N[0], k, (int64_t)m * k, 0, 0, 0, 0, 0, 0, ITB_MATMUL_B_CONST};
-    const char *pin = std::getenv("ITB_GEMM_IMPL");
-    if (!(pin && pin[0]) || !strcmp(pin, "tc")) {
+    if (g_sel_impl == SEL_AUTO || g_sel_impl == SEL_TC) {
         int r = launch_gemm_tc_grouped(dtype, g, n_groups, W, C, N, st);  // only when its tiles fill the machine (gate/up)
         if (r >= 0) return r;
     }
-    if (!(pin && pin[0]) || !strcmp(pin, "skinny")) {
+    if (g_sel_impl == SEL_AUTO || g_sel_impl == SEL_SKINNY) {
         int r = launch_gemm_skinny_grouped(dtype, g, n_groups, W, C, N, st);
         if (r >= 0) return r;
     }

@@ -52,7 +52,10 @@ int launch_gemm_skinny_grouped(int dtype, const GemmArgs &g0, int ngroups, const
 int launch_gemm_tc(int dtype, const GemmArgs &g, cudaStream_t st);
 int launch_gemm_tc_grouped(int dtype, const GemmArgs &g0, int ngroups, const void *const *Ws, void *const *Cs, const int *Ns,
                            cudaStream_t st);
-int tc_min_tiles_decode();  // column tiles (128 wide) from which a decode GEMM runs on the wgmma kernel instead of gemm_skinny
+// column tiles (128 wide) from which a decode GEMM (M <= 64) runs on the wgmma kernel instead of gemm_skinny: once its tiles alone
+// occupy every SM.  With fewer tiles gemm_skinny's cluster split-K spreads the weight stream over more SMs (tools/gemm_bench.py
+// compares the two)
+constexpr int TC_MIN_TILES_DECODE = kNumSMs;
 int launch_gemm_skinny_fp8w(int dtype, const GemmArgs &g0, int ngroups, const void *const *Wq, const float *const *scales,
                             void *const *Cs, const int *Ns, cudaStream_t st);
 

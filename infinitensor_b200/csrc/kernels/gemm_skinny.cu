@@ -17,8 +17,6 @@
 // Grid = ceil(N/64) x splitK CTAs, two co-resident per SM (~100 KB smem each).
 #include <cooperative_groups.h>
 
-#include <cstdlib>
-
 #include "gemm.cuh"
 
 namespace cg = cooperative_groups;
@@ -308,25 +306,15 @@ static int launch_skinny_nb(const GemmArgs &g, int ngroups, const void *const *W
         ITB_FAIL("matmul(skinny): cuTensorMapEncodeTiled(X) failed");
     const int ktiles = (g.k + SK_BK - 1) / SK_BK;
     // enough CTAs for two per SM, at least 4 k-tiles per CTA, cluster <= 8
-    static int target = 0;
-    if (!target) {
-        const char *e = std::getenv("ITB_SKINNY_TARGET_CTAS");
-        target = e && e[0] ? std::atoi(e) : 2 * kNumSMs;
-    }
-    int splitk = target / tiles_n;
+    int splitk = 2 * kNumSMs / tiles_n;
     splitk = std::max(1, std::min(splitk, 8));
     splitk = std::min(splitk, std::max(1, ktiles / 4));
     if (g_splitk_override) splitk = std::max(1, std::min(g_splitk_override, 8));
     int per = (ktiles + splitk - 1) / splitk;
     splitk = (ktiles + per - 1) / per;  // no empty split
 
-    static int budget_kb = 0;
-    if (!budget_kb) {
-        const char *e = std::getenv("ITB_SKINNY_SMEM_KB");
-        budget_kb = e && e[0] ? std::atoi(e) : 106;
-    }
-    const int stages = Cfg::stages_for(budget_kb);
-    const int smem_bytes = Cfg::smem_for(stages);
+    constexpr int stages = Cfg::stages_for(106);  // 106 KB per CTA: two CTAs per SM
+    constexpr int smem_bytes = Cfg::smem_for(stages);
     auto kern = gemm_skinny_kernel<T, MT, NB, W8>;
     {
         // the attribute is per DEVICE (a process may own runtimes on several GPUs): remember the largest request per device
@@ -364,14 +352,9 @@ static int launch_skinny_nb(const GemmArgs &g, int ngroups, const void *const *W
 template <typename T, int MT>
 static int launch_skinny_t(const GemmArgs &g, int ngroups, const void *const *Ws, void *const *Cs, const int *Ns,
                            cudaStream_t st) {
-    static int force = -1;
-    if (force < 0) {
-        const char *e = std::getenv("ITB_SKINNY_NB");
-        force = e && e[0] ? std::atoi(e) : 0;
-    }
     int tiles64 = 0;
     for (int i = 0; i < ngroups; ++i) tiles64 += (Ns[i] + 63) / 64;
-    const int nb = g_nb_override ? g_nb_override : force ? force : (tiles64 > 2 * kNumSMs ? 2 : 1);
+    const int nb = g_nb_override ? g_nb_override : (tiles64 > 2 * kNumSMs ? 2 : 1);
     if (nb == 2) return launch_skinny_nb<T, MT, 2>(g, ngroups, Ws, Cs, Ns, st);
     return launch_skinny_nb<T, MT, 1>(g, ngroups, Ws, Cs, Ns, st);
 }

@@ -18,8 +18,6 @@
 // Replaces the reference's cublasGemmEx dispatch (src/kernels/cuda/matmul.cc:141-168).
 #include <cooperative_groups.h>
 
-#include <cstdio>
-#include <cstdlib>
 #include <type_traits>
 
 #include "gemm.cuh"
@@ -33,20 +31,7 @@ constexpr int TC_W_BYTES = TC_BN * TC_BK * 2;  // 16 KB: two [64k x 64n] swizzle
 constexpr int TC_EPI_WARPS = 8;                      // two consumer warpgroups; in the epilogue two warps per 32-row quadrant
 constexpr int TC_THREADS = (TC_EPI_WARPS + 1) * 32;  // + TMA producer warp
 constexpr int TC_MAX_ROWS = 128;                     // rows of X per CTA (wgmma N): 16, 32, 64 or 128
-
-#ifdef ITB_TC_TRACE
-__device__ unsigned long long g_tc_trace[16];
-#define TC_MARK(i)                                                                         \
-    do {                                                                                   \
-        if (blockIdx.x == 0 && blockIdx.y == 0 && blockIdx.z == 0) {                       \
-            unsigned long long t_;                                                         \
-            asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t_));                         \
-            g_tc_trace[i] = t_;                                                            \
-        }                                                                                  \
-    } while (0)
-#else
-#define TC_MARK(i) do {} while (0)
-#endif
+constexpr int TC_SPLITK_MIN_KTILES = 24;             // k-tiles from which a GEMM on few CTAs is split over a cluster
 
 // 16 consecutive values -> two 16-byte stores (registers only: an address-taken T[16] costs a stack frame and 26 registers,
 // which halves the CTAs per SM of this kernel)
@@ -128,7 +113,6 @@ __global__ void __launch_bounds__(TC_THREADS, 2) gemm_tc_kernel(const __grid_con
     const int my_kt = max(0, kt_end - kt_begin);
 
     pdl_trigger();
-    if (threadIdx.x == 0) TC_MARK(0);
     if (threadIdx.x == 0) {
         for (int s = 0; s < S; ++s) {
             mbar_init(&full[s], 1);
@@ -141,7 +125,6 @@ __global__ void __launch_bounds__(TC_THREADS, 2) gemm_tc_kernel(const __grid_con
         tma_prefetch_desc(&mapX);
     }
     __syncthreads();
-    if (threadIdx.x == 0) TC_MARK(1);
 
     if (warp == TC_EPI_WARPS) {
         // ===== TMA producer (one thread; running ring slot / phase instead of it % S, it / S: a lone thread retires a dependent
@@ -163,9 +146,7 @@ __global__ void __launch_bounds__(TC_THREADS, 2) gemm_tc_kernel(const __grid_con
                     tma_load_3d(w_sm + it * TC_W_BYTES + TC_W_BYTES / 2, mapWp, &full[it], n0 + 64, k0, bw, pol_w);
                 }
             }
-            TC_MARK(2);
             pdl_wait();
-            TC_MARK(3);
             k0 = kt_begin * TC_BK;
             for (int it = 0; it < pre; ++it, k0 += TC_BK) tma_load_3d(x_sm + it * p.x_bytes, &mapX, &full[it], k0, m0, bx, pol_x);
             int s = 0;            // pre == S whenever the loop below runs
@@ -206,7 +187,6 @@ __global__ void __launch_bounds__(TC_THREADS, 2) gemm_tc_kernel(const __grid_con
             uint32_t ph = 0;
             for (int it = 0; it < my_kt; ++it) {
                 mbar_wait(&full[s], ph);
-                if (it == 0 && threadIdx.x == 0) TC_MARK(4);
                 const uint64_t a_desc = a_desc0 + (uint64_t)(s * a_st), b_desc = b_desc0 + (uint64_t)(s * b_st);
                 wg_fence();
 #pragma unroll
@@ -225,7 +205,6 @@ __global__ void __launch_bounds__(TC_THREADS, 2) gemm_tc_kernel(const __grid_con
         if (p.w_kmajor) mainloop(std::integral_constant<int, 0>{});
         else mainloop(std::integral_constant<int, 1>{});
         wg_wait<0>();
-        if (threadIdx.x == 0) TC_MARK(5);
         named_bar_sync(1, TC_EPI_WARPS * 32);  // both warpgroups are done with the ring: it holds the accumulator from here on
         acc_park<NT>(d, acc_sm, 64 * h);
         named_bar_sync(1, TC_EPI_WARPS * 32);
@@ -245,7 +224,6 @@ __global__ void __launch_bounds__(TC_THREADS, 2) gemm_tc_kernel(const __grid_con
             }
             asm volatile("bar.sync 1, %0;" ::"n"(TC_EPI_WARPS * 32) : "memory");
         }
-        if (threadIdx.x == 0) TC_MARK(6);
         // warp w reads accumulator rows [32 (w & 3), +32) = output columns n0 + 32 (w & 3) + lane; warps 0-3 take the first half
         // of the 16-row groups of X (accumulator columns), warps 4-7 the second
         const int quad = warp & 3;
@@ -357,7 +335,6 @@ __global__ void __launch_bounds__(TC_THREADS, 2) gemm_tc_kernel(const __grid_con
                 }
             }
         }
-        if (threadIdx.x == 0) TC_MARK(7);
     }
     if (nsplit > 1) {
         cluster.sync();
@@ -397,25 +374,6 @@ __global__ void __launch_bounds__(TC_THREADS, 2) gemm_tc_kernel(const __grid_con
     } else {
         __syncthreads();
     }
-    if (threadIdx.x == 0) TC_MARK(8);
-}
-
-int tc_splitk_min_ktiles() {
-    static const int v = [] {
-        const char *e = std::getenv("ITB_TC_SPLITK_MIN_KTILES");
-        return e && e[0] ? std::atoi(e) : 24;
-    }();
-    return v;
-}
-
-// decode GEMMs (M <= 64) take this kernel once its 128-column tiles alone occupy every SM; with fewer tiles the mma.sync kernel's
-// cluster split-K spreads the weight stream over more SMs (tools/gemm_bench.py compares the two)
-int tc_min_tiles_decode() {
-    static const int v = [] {
-        const char *e = std::getenv("ITB_TC_DECODE_MIN_TILES");
-        return e && e[0] ? std::atoi(e) : kNumSMs;
-    }();
-    return v;
 }
 
 template <typename T>
@@ -449,11 +407,11 @@ static int launch_tc_t(const GemmArgs &g, cudaStream_t st, bool is_bf16, int ngr
         splitk = (2 * kNumSMs) / tiles_n;
         splitk = std::max(1, std::min(splitk, 8));
         splitk = std::min(splitk, std::max(1, p.ktiles / 4));
-    } else if (p.mpad <= 128 && g.batch == 1 && !tail && !g.c_block && !g.c_nhwc && p.ktiles >= tc_splitk_min_ktiles() &&
+    } else if (p.mpad <= 128 && g.batch == 1 && !tail && !g.c_block && !g.c_nhwc && p.ktiles >= TC_SPLITK_MIN_KTILES &&
                tiles_n * p.m_chunks * 4 <= kNumSMs) {
         // a long serial k walk on a handful of CTAs (GPT-2's mlp c_proj: 48 k-tiles on 6 CTAs): split it over a cluster, >= 6 k-tiles each
         // (shorter walks -- the K = 768 projections -- stay unsplit: two cluster syncs and the DSMEM exchange cost about as much as the
-        //  k-tiles they save; ITB_TC_SPLITK_MIN_KTILES moves the threshold)
+        //  k-tiles they save)
         splitk = std::min(8, std::min(p.ktiles / 6, kNumSMs / (tiles_n * p.m_chunks)));
         splitk = std::max(1, splitk);
     }
@@ -461,15 +419,11 @@ static int launch_tc_t(const GemmArgs &g, cudaStream_t st, bool is_bf16, int ngr
     splitk = (p.ktiles + p.ktiles_per_split - 1) / p.ktiles_per_split;
     p.red_bytes = splitk > 1 ? p.mpad * TC_BN * 4 : 0;
     const int stage_bytes = TC_W_BYTES + p.x_bytes;
-    static const int budget_kb = [] {
-        const char *e = std::getenv("ITB_TC_SMEM_KB");
-        return e && e[0] ? std::atoi(e) : 0;
-    }();
     // a grid that cannot fill the SMs anyway (GPT-2's 6..24-tile projections) takes the whole shared memory for a deep ring:
     // one CTA per SM walking K serially is bound by bytes in flight / latency, so more stages help
     const bool small_grid = (int64_t)tiles_n * splitk * g.batch * p.m_chunks <= kNumSMs;
     // two CTAs per SM (<= 113 KB each): one CTA's epilogue overlaps the other's main loop
-    const int budget = (budget_kb ? budget_kb : p.mpad <= 64 ? 104 : small_grid ? 200 : 110) * 1024;
+    const int budget = (p.mpad <= 64 ? 104 : small_grid ? 200 : 110) * 1024;
     p.stages = std::max(2, std::min(8, (budget - p.red_bytes - 2048 - 16 * p.mpad) / stage_bytes));
     p.w_kmajor = g.trans_b ? 1 : 0;
     p.ring_bytes = std::max(p.stages * stage_bytes, p.mpad * ACC_LD * 4);
@@ -522,20 +476,6 @@ static int launch_tc_t(const GemmArgs &g, cudaStream_t st, bool is_bf16, int ngr
     cudaError_t e = cudaLaunchKernelEx(&cfg, kern, grp, mapX, g, p);
     ITB_CHECK(e == cudaSuccess, "matmul(wgmma): launch failed: %s", cudaGetErrorString(e));
     itb::count_launch();
-#ifdef ITB_TC_TRACE
-    {
-        static int n = 0;
-        if (++n % 16 == 0) {
-            cudaStreamSynchronize(st);
-            unsigned long long h[16];
-            cudaMemcpyFromSymbol(h, g_tc_trace, sizeof(h));
-            fprintf(stderr, "tc trace m=%d n=%d k=%d grid=(%d,%d,%d) stages=%d:", g.m, g.n, g.k, tiles_n, splitk,
-                    (int)(g.batch * p.m_chunks), p.stages);
-            for (int i = 1; i <= 8; ++i) fprintf(stderr, " t%d=%+.2fus", i, ((double)h[i] - (double)h[0]) / 1e3);
-            fprintf(stderr, "\n");
-        }
-    }
-#endif
     return 0;
 }
 
@@ -572,7 +512,7 @@ int launch_gemm_tc_grouped(int dtype, const GemmArgs &g0, int ngroups, const voi
         if (Ns[i] % 8 != 0 || Ns[i] < 64 || !aligned16(Ws[i]) || !aligned16(Cs[i])) return -1;
         tiles += (Ns[i] + TC_BN - 1) / TC_BN;
     }
-    if (tiles < tc_min_tiles_decode()) return -1;
+    if (tiles < TC_MIN_TILES_DECODE) return -1;
     GemmArgs g = g0;
     g.B = Ws[0];
     g.C = Cs[0];

@@ -43,29 +43,7 @@ int *stream_tickets(cudaStream_t st, int n) {
     return p;
 }
 long long launches() { return g_launches.load(std::memory_order_relaxed); }
-
-// L2 prefetch hint: "the kernel launched AFTER the next one will stream these bytes" -- consumed (and cleared) by the next launcher
-// that knows how to use it (the decode attention kernel; measured slower than no hint, see below -- opt-in)
-static thread_local const void *g_pf_ptr = nullptr;
-static thread_local long long g_pf_bytes = 0;
-void take_prefetch_hint(const void *&ptr, long long &bytes) {
-    // the attention kernel is latency-sensitive, and the extra traffic per layer can slow it by more than the o-projection gains from
-    // L2 (not measured on the H100).  Opt-in: ITB_L2_PREFETCH=1
-    static const bool off = [] {
-        const char *e = std::getenv("ITB_L2_PREFETCH");
-        return !(e && e[0] == '1');
-    }();
-    ptr = off ? nullptr : g_pf_ptr;
-    bytes = off ? 0 : g_pf_bytes;
-    g_pf_ptr = nullptr;
-    g_pf_bytes = 0;
-}
 }  // namespace itb
-
-extern "C" void it_b200_l2_prefetch_hint(const void *ptr, long long bytes) {
-    itb::g_pf_ptr = ptr;
-    itb::g_pf_bytes = ptr && bytes > 0 ? bytes : 0;
-}
 
 extern "C" const char *it_b200_last_error(void) { return itb::g_err; }
 extern "C" int it_b200_version(void) { return 1; }

@@ -1,8 +1,6 @@
 """GPU parity tests: every C-ABI launcher vs (a) the reference's golden vectors and (b) the CPU oracle
 on seeded inputs.  Tolerances are the ones SURVEY.md 8(c) states per op, written next to each check.
 Run with `pytest -m gpu` on an H100."""
-import os
-
 import numpy as np
 import pytest
 
@@ -281,10 +279,15 @@ SKINNY_SHAPES = [(16, 4096, 4096), (16, 4096, 11008), (16, 11008, 4096), (1, 256
 TC_SHAPES = SKINNY_SHAPES + [(128, 768, 2304), (128, 3072, 768), (200, 512, 640), (256, 1024, 1024), (96, 64, 128)]
 
 
+GEMM_IMPL = {"": 0, "skinny": 1, "tc": 2, "simt": 3}  # it_b200_matmul_select: "" = the production dispatch
+
+
 @pytest.fixture
-def gemm_impl(request, monkeypatch):
-    monkeypatch.setenv("ITB_GEMM_IMPL", request.param)
-    return request.param
+def gemm_impl(request):
+    from infinitensor_b200 import _lib
+    _lib.lib.it_b200_matmul_select(GEMM_IMPL[request.param], 0)
+    yield request.param
+    _lib.lib.it_b200_matmul_select(0, 0)
 
 
 def _gemm_case(K, m, k, n, dt):
@@ -322,15 +325,16 @@ def test_matmul_grouped_parity(K, gemm_impl, dt):
 def test_matmul_fused_epilogue_parity(K, dt):
     """MatMul + bias -> [Gelu] -> [+ residual] in the tcgen05 epilogue = the separate kernels (MatMul with bias, unary Gelu, binary
     Add), bit for bit -- the same fp32 sums and the same rounding points -- and the oracle chain within the GEMM tolerance."""
+    from infinitensor_b200 import _lib
     for ci, (m, k, n) in enumerate([(128, 768, 768), (128, 768, 3072), (128, 3072, 768), (200, 3072, 776), (65, 64, 64)]):  # (third: split-K cluster)
         a, b = rnd((m, k), 420 + ci, dt, 0.5), rnd((k, n), 430 + ci, dt, 0.05)
         bias, res = rnd((n,), 440 + ci, dt, 0.5), rnd((m, n), 450 + ci, dt)
         tol = gemm_tol(dt, k, np.abs(a).max(), np.abs(b).max())
-        os.environ["ITB_GEMM_IMPL"] = "tc"
+        _lib.lib.it_b200_matmul_select(GEMM_IMPL["tc"], 0)
         try:
             plain = K.matmul(a, b, bias, False, False, dt)
         finally:
-            os.environ.pop("ITB_GEMM_IMPL", None)
+            _lib.lib.it_b200_matmul_select(0, 0)
         for act, use_res in [(0, True), (4, False), (4, True), (1, True)]:
             got = K.matmul_fused(a, b, bias, res if use_res else None, act, dt)
             assert got is not None

@@ -30,7 +30,7 @@ def run(impl, m, k, n, reps=40, nbuf=12):
         e1.synchronize()
         us = e0.elapsed_time(e1) * 1e3 / reps
         return us, (k * n + m * (k + n)) * 2 / 1e9 / (us * 1e-6)
-    os.environ["ITB_GEMM_IMPL"] = impl
+    L.lib.it_b200_matmul_select({"skinny": 1, "tc": 2, "simt": 3}[impl], 0)
     ws = [torch.randn(k, n, device="cuda", dtype=torch.bfloat16) * 0.02 for _ in range(nbuf)]
     x = torch.randn(m, k, device="cuda", dtype=torch.bfloat16)
     y = torch.empty(m, n, device="cuda", dtype=torch.bfloat16)
@@ -48,6 +48,7 @@ def run(impl, m, k, n, reps=40, nbuf=12):
         go(i)
     e1.record()
     e1.synchronize()
+    L.lib.it_b200_matmul_select(0, 0)
     us = e0.elapsed_time(e1) * 1e3 / reps
     gb = (k * n + m * (k + n)) * 2 / 1e9
     return us, gb / (us * 1e-6)
