@@ -14,7 +14,7 @@
 //   * split-K across a thread-block CLUSTER (<= 8 CTAs along K): partial tiles are reduced by the
 //     rank-0 CTA through distributed shared memory, so there is no global workspace, no atomics
 //     and no second kernel; bias / activation / dtype conversion are fused into that store.
-// Grid = ceil(N/64) x splitK CTAs, two co-resident per SM (~100 KB smem each).
+// Grid = ceil(N/64) x splitK CTAs: unsplit, two co-resident per SM (~105 KB smem each); split-K, three (~65 KB each).
 #include <cooperative_groups.h>
 
 #include "gemm.cuh"
@@ -42,6 +42,12 @@ template <int MT, int NB, bool W8 = false> struct SkinnyCfg {
     }
     static constexpr int smem_for(int stages) { return stages * (W_BYTES + X_BYTES) + RED_BYTES + 2 * stages * 8 + 1024; }
 };
+
+// Ring budget of split-K launches (see launch_skinny_nb): three CTAs per SM.  An SM has 228 KB of shared memory and
+// reserves 1 KB per resident CTA.
+constexpr int kSkinnySplitBudgetKB = 66;
+constexpr int kSkinnySplitSmem = SkinnyCfg<1, 1>::smem_for(SkinnyCfg<1, 1>::stages_for(kSkinnySplitBudgetKB));
+static_assert(3 * (kSkinnySplitSmem + 1024) <= 228 * 1024, "split-K skinny GEMM: three CTAs must fit on one SM");
 
 // Up to 4 weight matrices that share the activation operand X (q/k/v, gate/up) run as ONE launch: the
 // N-tile index selects the group.  A plain MatMul is the 1-group case.
@@ -313,8 +319,16 @@ static int launch_skinny_nb(const GemmArgs &g, int ngroups, const void *const *W
     int per = (ktiles + splitk - 1) / splitk;
     splitk = (ktiles + per - 1) / per;  // no empty split
 
-    constexpr int stages = Cfg::stages_for(106);  // 106 KB per CTA: two CTAs per SM
-    constexpr int smem_bytes = Cfg::smem_for(stages);
+    // Unsplit launches: a 106 KB ring per CTA, two CTAs per SM, as many bytes in flight as the SM can hold.
+    // Split-K launches run as clusters, which are placed GPC by GPC: at two 106 KB CTAs per SM the 64 four-CTA clusters of
+    // a 4096-wide decode GEMM (o, down) took about twice their streaming time on H100, as a second wave of clusters would.
+    // A 66 KB ring lets three CTAs share an SM, and leaves room beside two of them for a gemm_tc CTA of the next GEMM
+    // (gate/up, logits), which then streams its first weight tiles under this kernel's tail (PDL).  FP8 weights keep the
+    // deep ring (measured slower at 66 KB).
+    constexpr int stages_deep = Cfg::stages_for(106);
+    constexpr int stages_split = W8 ? stages_deep : Cfg::stages_for(kSkinnySplitBudgetKB);
+    const int stages = splitk > 1 ? stages_split : stages_deep;
+    const int smem_bytes = Cfg::smem_for(stages);
     auto kern = gemm_skinny_kernel<T, MT, NB, W8>;
     {
         // the attribute is per DEVICE (a process may own runtimes on several GPUs): remember the largest request per device
