@@ -306,6 +306,16 @@ int it_b200_attention_kvcache_rope(int dtype, void *k_cache, void *v_cache, cons
                                    int rope_pos_dtype, void *out, int B, int H, int S_max, int D, void *workspace,
                                    int64_t workspace_bytes, void *stream);
 
+/* ---- AttentionKVCache with grouped-query attention: caches [B,Hkv,S_max,D], k/v [B,Hkv,1,D], q/out [B,Hq,1,D],
+ *      Hq = G * Hkv, G >= 1.  Query head i attends over KV head i / G (HF repeat_kv order); each K / V row is read once
+ *      for every 32 query heads of its group (once in all for G <= 32).  pos_flags as for it_b200_attention_kvcache; rope_pos NULL: no RoPE, else as the _rope
+ *      variant (q rotated per query head, k per KV head).  Workspace: it_b200_attention_kvcache_workspace(B, Hq, S_max, D).
+ *      Hq == Hkv launches exactly what it_b200_attention_kvcache / _rope launch. ---- */
+int it_b200_attention_kvcache_gqa(int dtype, void *k_cache, void *v_cache, const void *q, const void *k, const void *v,
+                                  const void *position_id, int pos_flags, const void *rope_pos, int rope_pos_dtype, void *out,
+                                  int B, int Hq, int Hkv, int S_max, int D, void *workspace, int64_t workspace_bytes,
+                                  void *stream);
+
 /* ---- Fused prefill attention (q-len > 1) on wgmma (SURVEY 8(f-3); attention_prefill.cu):
  *      out[b,h] = softmax((q . k^T) (/ or *) scale + mask) . v, q / k / v / out [B, H, S, D] f16 / bf16, D = 64 or 128.
  *      Replaces the chain the frontend lowers multi-token attention to -- Transpose(k) -> MatMul (matmul.cc:66-211) ->

@@ -515,10 +515,11 @@ void runAttentionRope(const Operator &ropeQ, const Operator &ropeK, const Operat
     auto qpre = ropeQ->getInputs(1), kpre = ropeK->getInputs(1), rpos = ropeQ->getInputs(0);
     IT_ASSERT(ropeK->getInputs(0) == rpos, "RoPE(q) and RoPE(k) must share the position tensor");
     const auto &d = kc->getDims();
-    int64_t wsb = it_b200_attention_kvcache_workspace(d[0], d[1], d[2], d[3]);
+    const int hq = att->getInputs(2)->getDims()[1];  // = G x the caches' d[1] KV heads
+    int64_t wsb = it_b200_attention_kvcache_workspace(d[0], hq, d[2], d[3]);
     void *ws = wsb ? RT(ctx)->getWorkspace((size_t)wsb) : nullptr;
-    CK(it_b200_attention_kvcache_rope(DTI(qpre), P(kc), P(vc), P(qpre), P(kpre), P(v), P(pos), attnPosFlags(att, rpos), P(rpos), DTI(rpos),
-                                      P(att->getOutput()), d[0], d[1], d[2], d[3], ws, wsb, S()), att);
+    CK(it_b200_attention_kvcache_gqa(DTI(qpre), P(kc), P(vc), P(qpre), P(kpre), P(v), P(pos), attnPosFlags(att, rpos), P(rpos),
+                                     DTI(rpos), P(att->getOutput()), d[0], hq, d[1], d[2], d[3], ws, wsb, S()), att);
 }
 
 void runPrefillAttention(const OpVec &ops, const RuntimeObj *) {
@@ -844,16 +845,16 @@ class AttentionKVCacheB200 : public CudaKernelWithoutConfig {
         auto kc = op->getInputs(0), vc = op->getInputs(1), q = op->getInputs(2), k = op->getInputs(3),
              v = op->getInputs(4), pos = op->getInputs(5);
         const auto &d = kc->getDims();
-        int64_t wsb = it_b200_attention_kvcache_workspace(d[0], d[1], d[2], d[3]);
+        const int hq = q->getDims()[1];  // = G x the caches' d[1] KV heads
+        int64_t wsb = it_b200_attention_kvcache_workspace(d[0], hq, d[2], d[3]);
         void *ws = wsb ? RT(ctx)->getWorkspace((size_t)wsb) : nullptr;
-        CK(it_b200_attention_kvcache(DTI(q), P(kc), P(vc), P(q), P(k), P(v), P(pos),
+        CK(it_b200_attention_kvcache_gqa(DTI(q), P(kc), P(vc), P(q), P(k), P(v), P(pos),
 #ifdef ITB_SEAM_A
-                                     DTI(pos) | (pos->getSource() || kc->getSource() || vc->getSource() ? ITB_POS_IN_STEP : 0),
+                                         DTI(pos) | (pos->getSource() || kc->getSource() || vc->getSource() ? ITB_POS_IN_STEP : 0),
 #else
-                                     b200::attnPosFlags(op, nullptr),
+                                         b200::attnPosFlags(op, nullptr),
 #endif
-                                     P(op->getOutput()), d[0],
-                                     d[1], d[2], d[3], ws, wsb, S()), op);
+                                         nullptr, 0, P(op->getOutput()), d[0], hq, d[1], d[2], d[3], ws, wsb, S()), op);
     }
 };
 

@@ -92,8 +92,15 @@ std::optional<vector<Shape>> AttentionKVCacheObj::inferShape(const TensorVec &in
     IT_ASSERT(ins.size() == 6);
     IT_ASSERT(ins[0]->getRank() == 4 && ins[2]->getRank() == 4, "AttentionKVCache expects rank-4 tensors");
     IT_ASSERT(ins[0]->getDims() == ins[1]->getDims(), "k_cache / v_cache shapes differ");
-    IT_ASSERT(ins[2]->getDims() == ins[3]->getDims() && ins[2]->getDims() == ins[4]->getDims(),
-              "q / k / v shapes differ");
+    IT_ASSERT(ins[3]->getDims() == ins[4]->getDims(), "k / v shapes differ");
+    IT_ASSERT(ins[3]->getRank() == 4, "AttentionKVCache expects rank-4 tensors");
+    // grouped-query attention: caches and k / v carry Hkv heads, q carries Hq = G * Hkv; query head i reads KV head i / G
+    const auto &c = ins[0]->getDims(), &q = ins[2]->getDims(), &k = ins[3]->getDims();
+    IT_ASSERT(q[0] == c[0] && k[0] == c[0], "AttentionKVCache: batch of q / k / v differs from the caches'");
+    IT_ASSERT(q[3] == c[3] && k[3] == c[3], "AttentionKVCache: head dim of q / k / v differs from the caches'");
+    IT_ASSERT(k[2] == q[2], "AttentionKVCache: q and k / v lengths differ");
+    IT_ASSERT(k[1] == c[1], "AttentionKVCache: k / v head count differs from the caches'");
+    IT_ASSERT(c[1] > 0 && q[1] % c[1] == 0, "AttentionKVCache: query heads are not a multiple of the caches' KV heads");
     return {{ins[2]->getDims()}};
 }
 

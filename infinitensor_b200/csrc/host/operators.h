@@ -61,6 +61,8 @@ class ConvObj : public OperatorObj {
     vector<int> getWorkloadVector() const override;
 };
 
+// caches [B, Hkv, S_max, D], q [B, Hq, S, D], k / v [B, Hkv, S, D], Hq % Hkv == 0; output shaped as q.  Grouped-query
+// attention (Hq = G Hkv, G > 1): query head i attends over KV head i / G, the order of HF's repeat_kv.
 class AttentionKVCacheObj : public OperatorObj {
     bool perRowPositions;  // extension (SURVEY 8(f-3)): row b attends up to position_id[b]; false = the reference's element-0 rule
 

@@ -144,6 +144,7 @@ static bool matchDecoderLayer(const vector<ExecStep> &s, size_t i, LayerMatch &m
     auto &cd = kc->getDims();
     if (cd.size() != 4 || cd[3] != 128 || cd[0] != rows || kc->getDType() != x->getDType()) return false;
     const int H = cd[1], dl = H * 128;
+    if (att->getInputs(2)->getDims()[1] != H) return false;  // grouped-query attention: the persistent kernel has one head count
     for (auto &mm : qkv)
         if (as<MatmulObj>(mm)->getN() != dl || as<MatmulObj>(mm)->getK() != d) return false;
     if (!soleUse(att->getOutput(), 1)) return false;
@@ -666,7 +667,8 @@ const vector<ExecStep> &GraphObj::getSchedule() {
             if (chain && t->getTargets().size() == 1 && t->getTargets()[0]->getOpType() == OpType::AttentionKVCache &&
                 xd.size() == 3 && xd[1] == 1 && xd[2] % 128 == 0 && op->getInputs(1)->getDType().isFloat()) {
                 auto att = t->getTargets()[0];
-                auto &qd = att->getInputs(2)->getDims();
+                // the operand this RoPE feeds: q carries Hq heads, k the caches' Hkv (fewer under grouped-query attention)
+                auto &qd = (att->getInputs(2) == t ? att->getInputs(2) : att->getInputs(3))->getDims();
                 if ((att->getInputs(2) == t || att->getInputs(3) == t) && qd[2] == 1 && qd[3] == 128 && qd[0] == xd[0] &&
                     qd[1] * 128 == xd[2]) {
                     deferredInto[att.get()].push_back(op);

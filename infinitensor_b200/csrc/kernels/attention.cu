@@ -408,6 +408,434 @@ __global__ void __launch_bounds__((WARPS + 1) * 32, AS_CTAS_PER_SM)
     }
 }
 
+// ------------------------------------------------------------------------------------------------------------------
+// attn_gqa_kernel: grouped-query decode, Hq = G x Hkv query heads with G > 1; query head i reads KV head i / G (HF
+// repeat_kv order).  The pipeline of attn_stream_kernel (flattened units in equal contiguous ranges over 2 x 132 CTAs,
+// cp.async.bulk producer, full/empty mbarrier ring, last-arriving CTA merges in CTA order) with the unit
+// (batch row, KV head, query group, 16 KiB chunk).  A query group is up to QT tiles of 16 query rows (rows past the
+// group's heads are zero padding): G <= 16 runs one tile, G > 16 groups of two, NQG = ceil(G / 32) groups per KV head.
+// For G <= 32 there is one group, so every K and V row is read from HBM once per step and used by all G query heads;
+// larger G (multi-query attention with 33+ heads) reads the KV head once per group.  Per chunk:
+//   S = Q K^T   warp w takes chunk rows [w CH/8, (w + 1) CH/8) of every query row -- mma.sync m16n8k16 with fp32
+//               accumulators for f16 / bf16, FFMA for fp32 -- and scales them by 1/sqrt(128) in fp32;
+//   softmax     the warps' row maxima and row sums meet in shared memory, every consumer derives the same running (m, l);
+//   O += P V    f16 / bf16: P enters the tensor core as two T operands, hi = P rounded to T and lo = P - hi rounded to T
+//               (two MMAs), so each weight keeps 16 (bf16) / 22 (f16) significant bits instead of T's 8 / 11 -- rounding P
+//               once, as FlashAttention does, was measured at up to 2 ulp of bf16 off the oracle on short contexts.
+//               Warp w owns output columns [16w, 16w + 16) of every query row, so O is never merged across warps.
+// The row appended this step is stored into the ring slot after the last chunk's cache rows and takes part in that
+// chunk's products like any other row; group 0 also stores it in place.
+// ------------------------------------------------------------------------------------------------------------------
+constexpr int GQ_WARPS = 8;
+
+template <typename T> struct GqaCfg {
+    static constexpr int CH = 16384 / (kD * (int)sizeof(T));  // cache rows per 16 KiB chunk: 64 (f16 / bf16), 32 (fp32)
+    static constexpr int NC = CH / (GQ_WARPS * 4);            // S columns per thread: 2, 1
+    static constexpr int QLD = kD + 16 / (int)sizeof(T);      // +16 B per row: ldmatrix rows fall in distinct banks
+    static constexpr int PLD = CH + 16 / (int)sizeof(T);
+};
+
+template <typename T, int QT, bool ROPE>
+__global__ void __launch_bounds__((GQ_WARPS + 1) * 32, AS_CTAS_PER_SM)
+    attn_gqa_kernel(T *__restrict__ kcache, T *__restrict__ vcache, const T *__restrict__ q,
+                    const T *__restrict__ kin, const T *__restrict__ vin, const void *__restrict__ position_id,
+                    int pos_flags, T *__restrict__ out, int Smax, int Bn, int Hkv, int G, int NQG,
+                    float *__restrict__ partial, int slots_per_head, int *__restrict__ tickets, const void *__restrict__ rope_pos, int rope_pos_dtype) {
+    using C = RowCfg<T>;
+    using Q = GqaCfg<T>;
+    constexpr int EPL = C::EPL, LPR = C::LPR, RPW = C::RPW;
+    constexpr int CH = Q::CH, NC = Q::NC, QLD = Q::QLD, PLD = Q::PLD;
+    constexpr int GP = 16 * QT;  // padded query rows
+    constexpr int CHUNK_BYTES = CH * kD * (int)sizeof(T);
+    constexpr int CONSUMERS = GQ_WARPS * 32;
+    constexpr bool MMA = sizeof(T) == 2;
+    constexpr float kScale = 0.08838834764831845f;  // 1/sqrt(128)
+    extern __shared__ __align__(128) unsigned char ring[];  // stages x { K chunk | V chunk }
+    __shared__ __align__(8) uint64_t full[AS_STAGES], empty[AS_STAGES];
+    __shared__ __align__(16) T s_q[GP * QLD];   // (rotated) query rows of the current query group
+    __shared__ __align__(16) T s_p[GP * PLD];   // P of the current chunk, rounded to T
+    __shared__ __align__(16) T s_plo[MMA ? GP * PLD : 1];  // f16 / bf16: P - s_p, rounded to T
+    __shared__ float s_red[2][GQ_WARPS][GP];    // per-warp row maxima / row sums of the current chunk
+    __shared__ float s_cs[kD / 2], s_sn[kD / 2];
+    __shared__ int s_last;
+    __shared__ int s_pre[AS_MAX_B + 1];  // (KV head, query group, chunk) units before batch row b; s_pre[B] = total
+
+    pdl_trigger();
+    const int pos_dtype = pos_flags & 0xff;
+    const bool per_row = (pos_flags & ITB_POS_PER_ROW) != 0;
+    if (pos_flags & ITB_POS_IN_STEP) pdl_wait();  // (see attn_stream_kernel)
+    auto pos_of = [&](int b) {
+        const int p = pos_dtype == ITB_I64 ? read_pos<int64_t>(position_id, per_row ? b : 0)
+                                           : read_pos<int32_t>(position_id, per_row ? b : 0);
+        return min(max(p, 0), Smax - 1);
+    };
+    if (threadIdx.x == 0) {
+        for (int s = 0; s < AS_STAGES; ++s) {
+            mbar_init(&full[s], 1);
+            mbar_init(&empty[s], GQ_WARPS);
+        }
+        fence_mbar_init();
+    }
+    // V rows past a chunk's valid rows enter the P.V product with P = 0: they must hold finite values, so the ring starts
+    // zeroed (later it only ever holds cache rows)
+    for (int i = threadIdx.x; i < AS_STAGES * 2 * CHUNK_BYTES / 16; i += blockDim.x)
+        reinterpret_cast<uint4 *>(ring)[i] = make_uint4(0, 0, 0, 0);
+    fence_proxy_async();
+    const int HV = Hkv * NQG;  // (KV head, query group) segments per batch row
+    for (int b = threadIdx.x; b < Bn; b += blockDim.x) s_pre[b] = HV * (pos_of(b) / CH + 1);
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        int acc = 0;
+        for (int b = 0; b < Bn; ++b) {
+            const int n = s_pre[b];
+            s_pre[b] = acc;
+            acc += n;
+        }
+        s_pre[Bn] = acc;
+    }
+    __syncthreads();
+
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int BH = Bn * HV;
+    const int64_t total = s_pre[Bn], ncta = min((int64_t)gridDim.x, total);
+    if (blockIdx.x >= ncta) return;
+    int nunits, bh, c, brow, pos, nch;  // bh = (b * Hkv + KV head) * NQG + query group
+    {
+        const int64_t u0 = blockIdx.x * total / ncta, u1 = (blockIdx.x + 1) * total / ncta;
+        nunits = (int)(u1 - u0);
+        brow = 0;
+        while (brow + 1 < Bn && s_pre[brow + 1] <= u0) ++brow;
+        pos = pos_of(brow);
+        nch = pos / CH + 1;
+        const int r = (int)(u0 - s_pre[brow]);
+        bh = brow * HV + r / nch;
+        c = r % nch;
+    }
+    auto next_unit = [&]() {
+        if (++c == nch) {
+            c = 0;
+            ++bh;
+            if (bh % HV == 0 && bh < BH) {
+                brow = bh / HV;
+                pos = pos_of(brow);
+                nch = pos / CH + 1;
+            }
+        }
+    };
+
+    if (warp == GQ_WARPS) {
+        // ---------------- producer (as attn_stream_kernel) ----------------
+        if (lane == 0) {
+            const uint64_t policy = l2_policy_evict_first();
+            int st = 0, ph = 0;
+            for (int it = 0; it < nunits; ++it) {
+                mbar_wait(&empty[st], ph ^ 1);
+                const int rows = min(CH, pos - c * CH);
+                if (rows > 0) {
+                    const uint32_t bytes = (uint32_t)rows * kD * (uint32_t)sizeof(T);
+                    const int64_t off = ((int64_t)(bh / NQG) * Smax + (int64_t)c * CH) * kD;
+                    mbar_expect_tx(&full[st], 2 * bytes);
+                    bulk_load_1d(ring + (size_t)st * 2 * CHUNK_BYTES, kcache + off, bytes, &full[st], policy);
+                    bulk_load_1d(ring + (size_t)st * 2 * CHUNK_BYTES + CHUNK_BYTES, vcache + off, bytes, &full[st], policy);
+                } else {
+                    mbar_arrive(&full[st]);
+                }
+                next_unit();
+                if (++st == AS_STAGES) { st = 0; ph ^= 1; }
+            }
+        }
+        return;
+    }
+
+    // ---------------- consumers ----------------
+    int table_b = -1;
+    auto rope_table = [&](int b) {
+        if (threadIdx.x < kD / 2) {
+            const float p = rope_pos_dtype == ITB_I64 ? (float)(int)((const int64_t *)rope_pos)[b]
+                                                      : (float)((const int32_t *)rope_pos)[b];
+            const float freq = p * powf(10000.f, -(float)(threadIdx.x * 2) / (float)kD);
+            s_cs[threadIdx.x] = round_t<T>(cosf(freq));
+            s_sn[threadIdx.x] = round_t<T>(sinf(freq));
+        }
+        named_bar_sync(1, CONSUMERS);
+        table_b = b;
+    };
+    if (ROPE) rope_table(bh / HV);
+    pdl_wait();
+    const int sub = lane / LPR, col = (lane % LPR) * EPL;  // row-load layout (q, appended k / v)
+    const int qr = lane >> 2, qc = lane & 3;               // fragment layout: rows qr, qr + 8 of each 16-row tile
+    const int cw = warp * (CH / GQ_WARPS);                 // first chunk row of this warp's S columns
+    float m_run[QT][2], l_run[QT][2], o[QT][2][4];         // o[t][j][2h + e]: row 16t + qr + 8h, column 16w + 8j + 2qc + e
+    bool seg_from_start = false;
+    int st = 0, ph = 0;
+    int64_t q0 = 0;  // first query head of the segment's group
+    int gq = 0;      // query heads in the segment's group (<= GP)
+    for (int it = 0; it < nunits; ++it) {
+        if (it == 0 || c == 0) {
+            // new segment: reset the running softmax, stage the group's query rows (rotated if asked)
+            seg_from_start = c == 0;
+#pragma unroll
+            for (int t = 0; t < QT; ++t)
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                    m_run[t][h] = -INFINITY;
+                    l_run[t][h] = 0.f;
+#pragma unroll
+                    for (int j = 0; j < 2; ++j) o[t][j][2 * h] = o[t][j][2 * h + 1] = 0.f;
+                }
+            if (ROPE && bh / HV != table_b) rope_table(bh / HV);
+            // query heads [kvh G + qg GP, + gq) of batch row b
+            q0 = (int64_t)(bh / NQG) * G + (int64_t)(bh % NQG) * GP;
+            gq = min(GP, G - (bh % NQG) * GP);
+            const T *qh = q + q0 * kD;
+            for (int r0 = warp * RPW; r0 < GP; r0 += GQ_WARPS * RPW) {
+                const int r = r0 + sub;
+                Vec16<T> x;
+                *reinterpret_cast<uint4 *>(x.v) = make_uint4(0, 0, 0, 0);
+                if (r < gq) x = ld16(qh + (int64_t)r * kD + col);
+                if (ROPE) rope_one<T, EPL, LPR>(x, col, s_cs, s_sn);
+                st16(s_q + r * QLD + col, x);
+            }
+            named_bar_sync(1, CONSUMERS);
+        }
+        const int nvalid = pos - c * CH;  // cache rows of this chunk below the position (last chunk: < CH)
+        const bool last_chunk = c == nch - 1;
+        T *ks = reinterpret_cast<T *>(ring + (size_t)st * 2 * CHUNK_BYTES), *vs = ks + CH * kD;
+        mbar_wait(&full[st], ph);
+        int nrows = min(nvalid, CH);
+        if (last_chunk) {
+            // the row appended this step: rotate k if asked, store k / v into ring row nvalid, and (group 0) in place
+            if (warp == 0) {
+                const int64_t kv = bh / NQG;
+#pragma unroll
+                for (int r0 = 0; r0 < 2; r0 += RPW) {
+                    const int which = r0 + sub;  // 0: k, 1: v
+                    Vec16<T> x = ld16((which == 0 ? kin : vin) + kv * kD + col);
+                    if (ROPE) {
+                        Vec16<T> xr = x;
+                        rope_one<T, EPL, LPR>(xr, col, s_cs, s_sn);
+                        if (which == 0) x = xr;
+                    }
+                    if (bh % NQG == 0) st16((which == 0 ? kcache : vcache) + (kv * Smax + pos) * kD + col, x);
+                    st16((which == 0 ? ks : vs) + nvalid * kD + col, x);
+                }
+                fence_proxy_async();  // the producer's next bulk copy into this stage must land after these stores
+            }
+            named_bar_sync(1, CONSUMERS);
+            nrows = nvalid + 1;
+        }
+
+        // ---- S = Q K^T for this warp's chunk rows, scaled, masked past nrows: s[t][h][e] = S[16t + qr + 8h][cw + NC qc + e]
+        float s[QT][2][NC];
+        if constexpr (MMA) {
+            uint32_t kf[8][2];
+#pragma unroll
+            for (int jj = 0; jj < 4; ++jj)
+                ldmatrix_x4(kf[2 * jj][0], kf[2 * jj][1], kf[2 * jj + 1][0], kf[2 * jj + 1][1],
+                            smem_u32(ks + (cw + (lane & 7)) * kD + 32 * jj + 8 * (lane >> 3)));
+#pragma unroll
+            for (int t = 0; t < QT; ++t) {
+                float acc[4] = {0.f, 0.f, 0.f, 0.f};
+#pragma unroll
+                for (int kk = 0; kk < 8; ++kk) {
+                    uint32_t a[4];
+                    ldmatrix_x4(a[0], a[1], a[2], a[3], smem_u32(s_q + (16 * t + (lane & 15)) * QLD + 16 * kk + 8 * (lane >> 4)));
+                    mma_m16n8k16<T>(acc, a, kf[kk][0], kf[kk][1]);
+                }
+#pragma unroll
+                for (int h = 0; h < 2; ++h)
+#pragma unroll
+                    for (int e = 0; e < 2; ++e) s[t][h][e] = acc[2 * h + e] * kScale;
+            }
+        } else {
+            const float *kr = reinterpret_cast<const float *>(ks) + (cw + qc) * kD;
+#pragma unroll
+            for (int t = 0; t < QT; ++t)
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                    const float *qrow = reinterpret_cast<const float *>(s_q) + (16 * t + qr + 8 * h) * QLD;
+                    float d = 0.f;
+#pragma unroll 8
+                    for (int dd = 0; dd < kD; dd += 4) {
+                        const float4 a = *reinterpret_cast<const float4 *>(qrow + dd);
+                        const float4 b = *reinterpret_cast<const float4 *>(kr + dd);
+                        d = fmaf(a.x, b.x, d);
+                        d = fmaf(a.y, b.y, d);
+                        d = fmaf(a.z, b.z, d);
+                        d = fmaf(a.w, b.w, d);
+                    }
+                    s[t][h][0] = d * kScale;
+                }
+        }
+        // ---- softmax: chunk row maxima across the warps, then P and its row sums
+#pragma unroll
+        for (int t = 0; t < QT; ++t)
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                float mx = -INFINITY;
+#pragma unroll
+                for (int e = 0; e < NC; ++e) {
+                    if (cw + NC * qc + e >= nrows) s[t][h][e] = -INFINITY;
+                    mx = fmaxf(mx, s[t][h][e]);
+                }
+                mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+                mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+                if (qc == 0) s_red[0][warp][16 * t + qr + 8 * h] = mx;
+            }
+        named_bar_sync(1, CONSUMERS);
+        float corr[QT][2];
+#pragma unroll
+        for (int t = 0; t < QT; ++t)
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                const int r = 16 * t + qr + 8 * h;
+                float cm = -INFINITY;
+#pragma unroll
+                for (int w = 0; w < GQ_WARPS; ++w) cm = fmaxf(cm, s_red[0][w][r]);
+                const float mnew = fmaxf(m_run[t][h], cm);  // finite: every chunk has >= 1 row
+                float sum = 0.f;
+                __align__(4) T hi[NC], lo[NC];
+#pragma unroll
+                for (int e = 0; e < NC; ++e) {
+                    const float p = expf(s[t][h][e] - mnew);  // masked: exp(-inf) = 0
+                    hi[e] = from_f<T>(p);
+                    lo[e] = from_f<T>(p - to_f(hi[e]));
+                    sum += p;
+                }
+                if constexpr (MMA) {
+                    *reinterpret_cast<uint32_t *>(s_p + r * PLD + cw + NC * qc) = *reinterpret_cast<const uint32_t *>(hi);
+                    *reinterpret_cast<uint32_t *>(s_plo + r * PLD + cw + NC * qc) = *reinterpret_cast<const uint32_t *>(lo);
+                } else {
+                    s_p[r * PLD + cw + qc] = hi[0];
+                }
+                sum += __shfl_xor_sync(0xffffffffu, sum, 1);
+                sum += __shfl_xor_sync(0xffffffffu, sum, 2);
+                if (qc == 0) s_red[1][warp][r] = sum;
+                corr[t][h] = expf(m_run[t][h] - mnew);  // m_run = -inf -> 0
+                m_run[t][h] = mnew;
+            }
+        named_bar_sync(1, CONSUMERS);
+#pragma unroll
+        for (int t = 0; t < QT; ++t)
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                float ls = 0.f;
+#pragma unroll
+                for (int w = 0; w < GQ_WARPS; ++w) ls += s_red[1][w][16 * t + qr + 8 * h];
+                l_run[t][h] = l_run[t][h] * corr[t][h] + ls;
+#pragma unroll
+                for (int j = 0; j < 2; ++j) {
+                    o[t][j][2 * h] *= corr[t][h];
+                    o[t][j][2 * h + 1] *= corr[t][h];
+                }
+            }
+        // ---- O += P V over output columns [16w, 16w + 16)
+        if constexpr (MMA) {
+#pragma unroll
+            for (int kk = 0; kk < CH / 16; ++kk) {
+                uint32_t b0, b1, b2, b3;
+                ldmatrix_x4_trans(b0, b1, b2, b3,
+                                  smem_u32(vs + (16 * kk + (lane & 7) + 8 * ((lane >> 3) & 1)) * kD + 16 * warp + 8 * (lane >> 4)));
+#pragma unroll
+                for (int t = 0; t < QT; ++t) {
+                    const int off = (16 * t + (lane & 15)) * PLD + 16 * kk + 8 * (lane >> 4);
+                    uint32_t a[4];
+                    ldmatrix_x4(a[0], a[1], a[2], a[3], smem_u32(s_plo + off));
+                    mma_m16n8k16<T>(o[t][0], a, b0, b1);
+                    mma_m16n8k16<T>(o[t][1], a, b2, b3);
+                    ldmatrix_x4(a[0], a[1], a[2], a[3], smem_u32(s_p + off));
+                    mma_m16n8k16<T>(o[t][0], a, b0, b1);
+                    mma_m16n8k16<T>(o[t][1], a, b2, b3);
+                }
+            }
+        } else {
+            const float *vcol = reinterpret_cast<const float *>(vs) + 16 * warp + 2 * qc;
+            const float *pf = reinterpret_cast<const float *>(s_p);
+            for (int k = 0; k < nrows; ++k) {
+                const float2 v0 = *reinterpret_cast<const float2 *>(vcol + k * kD);
+                const float2 v1 = *reinterpret_cast<const float2 *>(vcol + k * kD + 8);
+#pragma unroll
+                for (int t = 0; t < QT; ++t)
+#pragma unroll
+                    for (int h = 0; h < 2; ++h) {
+                        const float p = pf[(16 * t + qr + 8 * h) * PLD + k];
+                        o[t][0][2 * h] = fmaf(p, v0.x, o[t][0][2 * h]);
+                        o[t][0][2 * h + 1] = fmaf(p, v0.y, o[t][0][2 * h + 1]);
+                        o[t][1][2 * h] = fmaf(p, v1.x, o[t][1][2 * h]);
+                        o[t][1][2 * h + 1] = fmaf(p, v1.y, o[t][1][2 * h + 1]);
+                    }
+            }
+        }
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&empty[st]);
+        if (++st == AS_STAGES) { st = 0; ph ^= 1; }
+
+        if (last_chunk || it == nunits - 1) {
+            // ---- segment end: write O / l, or this CTA's partial; the last CTA of a shared segment merges its gq rows
+            const bool whole = seg_from_start && last_chunk;
+            const int64_t hu0 = (int64_t)s_pre[brow] + (int64_t)(bh - brow * HV) * nch;  // first unit of this segment
+            const int first_cta = (int)(((hu0 + 1) * ncta - 1) / total);
+            const int last_cta = (int)(((hu0 + nch) * ncta - 1) / total);
+            const int nseg = last_cta - first_cta + 1;
+#pragma unroll
+            for (int t = 0; t < QT; ++t)
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                    const int r = 16 * t + qr + 8 * h;
+                    if (r >= gq) continue;
+                    if (whole) {
+                        T *orow = out + (q0 + r) * kD + 16 * warp + 2 * qc;
+#pragma unroll
+                        for (int j = 0; j < 2; ++j) {
+                            orow[8 * j] = from_f<T>(o[t][j][2 * h] / l_run[t][h]);
+                            orow[8 * j + 1] = from_f<T>(o[t][j][2 * h + 1] / l_run[t][h]);
+                        }
+                    } else {
+                        float *pp = partial + ((q0 + r) * slots_per_head + ((int)blockIdx.x - first_cta)) * (kD + 2);
+#pragma unroll
+                        for (int j = 0; j < 2; ++j) {
+                            __stcg(pp + 2 + 16 * warp + 8 * j + 2 * qc, o[t][j][2 * h]);
+                            __stcg(pp + 2 + 16 * warp + 8 * j + 2 * qc + 1, o[t][j][2 * h + 1]);
+                        }
+                        if (warp == 0 && qc == 0) {
+                            __stcg(pp, m_run[t][h]);
+                            __stcg(pp + 1, l_run[t][h]);
+                        }
+                    }
+                }
+            if (!whole) {
+                __threadfence();
+                named_bar_sync(1, CONSUMERS);
+                if (threadIdx.x == 0) {
+                    const int old = atomicAdd(tickets + bh, 1);
+                    s_last = old == nseg - 1;
+                    if (s_last) tickets[bh] = 0;  // self-cleaning: every other sharer has already arrived
+                    __threadfence();
+                }
+                named_bar_sync(1, CONSUMERS);
+                if (s_last) {
+                    for (int i = threadIdx.x; i < gq * kD; i += CONSUMERS) {
+                        const int r = i / kD, d = i % kD;
+                        const float *slots = partial + (q0 + r) * slots_per_head * (kD + 2);
+                        float mw = -INFINITY;
+                        for (int s2 = 0; s2 < nseg; ++s2) mw = fmaxf(mw, __ldcg(slots + (int64_t)s2 * (kD + 2)));
+                        float L = 0.f, A = 0.f;
+                        for (int s2 = 0; s2 < nseg; ++s2) {
+                            const float *pp = slots + (int64_t)s2 * (kD + 2);
+                            const float cw2 = expf(__ldcg(pp) - mw);  // every partial holds >= 1 row: finite m
+                            L += __ldcg(pp + 1) * cw2;
+                            A += __ldcg(pp + 2 + d) * cw2;
+                        }
+                        out[(q0 + r) * kD + d] = from_f<T>(A / L);
+                    }
+                }
+            }
+            named_bar_sync(1, CONSUMERS);  // s_q / s_last are reused by the next segment
+        }
+        next_unit();
+    }
+}
+
 }  // namespace itb
 
 using namespace itb;
@@ -438,9 +866,44 @@ static int launch_attn_stream(T *kc, T *vc, const T *q, const T *k, const T *v, 
     return e == cudaSuccess ? 0 : 1;
 }
 
+template <typename T, int QT, bool ROPE>
+static int launch_attn_gqa(T *kc, T *vc, const T *q, const T *k, const T *v, const void *position_id, int pos_flags,
+                           const void *rope_pos, int rope_pos_dtype, T *out, int B, int Hkv, int G, int S_max,
+                           float *workspace, cudaStream_t st) {
+    constexpr int CH = GqaCfg<T>::CH;
+    const size_t smem = (size_t)AS_STAGES * 2 * CH * kD * sizeof(T);
+    auto kern = attn_gqa_kernel<T, QT, ROPE>;
+    if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) return 1;
+    const int nqg = (G + 16 * QT - 1) / (16 * QT);  // query groups per KV head
+    int *tickets = stream_tickets(st, B * Hkv * nqg);
+    if (!tickets) return 1;
+    const int64_t max_units = (int64_t)B * Hkv * nqg * (S_max / CH + 1);
+    const int grid = (int)std::min<int64_t>(max_units, (int64_t)AS_CTAS_PER_SM * kNumSMs);
+    cudaError_t e = launch_k(kern, dim3(grid), dim3((GQ_WARPS + 1) * 32), smem, st, kc, vc, q, k, v, position_id, pos_flags,
+                             out, S_max, B, Hkv, G, nqg, workspace, stream_slots_per_head(S_max), tickets, rope_pos,
+                             rope_pos_dtype);
+    return e == cudaSuccess ? 0 : 1;
+}
+
+// one query tile of 16 rows for G <= 16, else groups of two tiles (four tiles spill registers and, for fp32, exceed the
+// static shared memory)
+template <typename T, bool ROPE>
+static int launch_attn_gqa_tiles(T *kc, T *vc, const T *q, const T *k, const T *v, const void *position_id, int pos_flags,
+                                 const void *rope_pos, int rope_pos_dtype, T *out, int B, int Hkv, int G, int S_max,
+                                 float *workspace, cudaStream_t st) {
+    if (G <= 16)
+        return launch_attn_gqa<T, 1, ROPE>(kc, vc, q, k, v, position_id, pos_flags, rope_pos, rope_pos_dtype, out, B, Hkv, G,
+                                           S_max, workspace, st);
+    return launch_attn_gqa<T, 2, ROPE>(kc, vc, q, k, v, position_id, pos_flags, rope_pos, rope_pos_dtype, out, B, Hkv, G,
+                                       S_max, workspace, st);
+}
+
+// Hq query heads over Hkv cache heads.  Hq == Hkv runs attn_stream_kernel; Hq = G Hkv, G > 1, runs attn_gqa_kernel.
 static int attention_impl(int dtype, void *k_cache, void *v_cache, const void *q, const void *k, const void *v,
                           const void *position_id, int pos_flags, const void *rope_pos, int rope_pos_dtype, void *out,
-                          int B, int H, int S_max, int D, void *workspace, int64_t workspace_bytes, void *stream) {
+                          int B, int Hq, int Hkv, int S_max, int D, void *workspace, int64_t workspace_bytes,
+                          void *stream) {
+    const int H = Hq;
     const int pos_dtype = pos_flags & 0xff;
     ITB_CHECK(D == kD, "AttentionKVCache: head dim %d != 128 (reference attention_kvcache.cu:154)", D);
     ITB_CHECK(pos_dtype == ITB_I32 || pos_dtype == ITB_U32 || pos_dtype == ITB_I64,
@@ -451,12 +914,29 @@ static int attention_impl(int dtype, void *k_cache, void *v_cache, const void *q
               "AttentionKVCache: tensors must be 16-byte aligned");
     const int BH = B * H;
     if (BH == 0) return 0;
+    ITB_CHECK(Hkv > 0 && Hq % Hkv == 0, "AttentionKVCache: %d query heads are not a multiple of %d KV heads", Hq, Hkv);
+    const int G = Hq / Hkv;
     ITB_CHECK(B <= AS_MAX_B && BH <= 65536, "AttentionKVCache: batch %d x heads %d beyond the kernel's limits (%d rows, 65536 heads)",
               B, H, AS_MAX_B);
     const int64_t need = it_b200_attention_kvcache_workspace(B, H, S_max, D);
     ITB_CHECK(workspace && workspace_bytes >= need, "AttentionKVCache: workspace %lld < %lld bytes",
               (long long)workspace_bytes, (long long)need);
     auto st = (cudaStream_t)stream;
+    if (G > 1) {
+        ITB_DISPATCH_FLOAT(dtype, "AttentionKVCache", {
+            int rc = rope_pos ? launch_attn_gqa_tiles<T, true>((T *)k_cache, (T *)v_cache, (const T *)q, (const T *)k,
+                                                               (const T *)v, position_id, pos_flags, rope_pos,
+                                                               rope_pos_dtype, (T *)out, B, Hkv, G, S_max,
+                                                               (float *)workspace, st)
+                              : launch_attn_gqa_tiles<T, false>((T *)k_cache, (T *)v_cache, (const T *)q, (const T *)k,
+                                                                (const T *)v, position_id, pos_flags, nullptr, 0,
+                                                                (T *)out, B, Hkv, G, S_max, (float *)workspace, st);
+            ITB_CHECK(rc == 0, "AttentionKVCache: grouped-query kernel launch failed: %s",
+                      cudaGetErrorString(cudaGetLastError()));
+            ITB_LAUNCH_CHECK("AttentionKVCache");
+        });
+        return 0;
+    }
     ITB_DISPATCH_FLOAT(dtype, "AttentionKVCache", {
         int rc = rope_pos ? launch_attn_stream<T, true>((T *)k_cache, (T *)v_cache, (const T *)q, (const T *)k,
                                                         (const T *)v, position_id, pos_flags, rope_pos,
@@ -475,8 +955,16 @@ extern "C" int it_b200_attention_kvcache(int dtype, void *k_cache, void *v_cache
                                          const void *v, const void *position_id, int pos_dtype, void *out, int B,
                                          int H, int S_max, int D, void *workspace, int64_t workspace_bytes,
                                          void *stream) {
-    return attention_impl(dtype, k_cache, v_cache, q, k, v, position_id, pos_dtype, nullptr, 0, out, B, H, S_max, D,
+    return attention_impl(dtype, k_cache, v_cache, q, k, v, position_id, pos_dtype, nullptr, 0, out, B, H, H, S_max, D,
                           workspace, workspace_bytes, stream);
+}
+
+extern "C" int it_b200_attention_kvcache_gqa(int dtype, void *k_cache, void *v_cache, const void *q, const void *k,
+                                             const void *v, const void *position_id, int pos_flags, const void *rope_pos,
+                                             int rope_pos_dtype, void *out, int B, int Hq, int Hkv, int S_max, int D,
+                                             void *workspace, int64_t workspace_bytes, void *stream) {
+    return attention_impl(dtype, k_cache, v_cache, q, k, v, position_id, pos_flags, rope_pos, rope_pos_dtype, out, B, Hq,
+                          Hkv, S_max, D, workspace, workspace_bytes, stream);
 }
 
 extern "C" int it_b200_attention_kvcache_rope(int dtype, void *k_cache, void *v_cache, const void *q_pre,
@@ -485,5 +973,5 @@ extern "C" int it_b200_attention_kvcache_rope(int dtype, void *k_cache, void *v_
                                               int S_max, int D, void *workspace, int64_t workspace_bytes, void *stream) {
     ITB_CHECK(rope_pos != nullptr, "AttentionKVCache+RoPE: rope positions missing");
     return attention_impl(dtype, k_cache, v_cache, q_pre, k_pre, v, position_id, pos_dtype, rope_pos, rope_pos_dtype, out,
-                          B, H, S_max, D, workspace, workspace_bytes, stream);
+                          B, H, H, S_max, D, workspace, workspace_bytes, stream);
 }

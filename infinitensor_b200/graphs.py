@@ -66,6 +66,17 @@ class LlamaConfig:
     batch: int = 16
     dtype: int = BF16
     fp8_weights: bool = False  # the seven projection matrices of every layer + the logits head as FP8 E4M3 codes + f32 column scales
+    kv_heads: int | None = None  # grouped-query attention: KV heads shared by heads // kv_heads query heads each; None = heads
+
+    @property
+    def n_kv(self) -> int:
+        return self.heads if self.kv_heads is None else self.kv_heads
+
+    @staticmethod
+    def llama3_8b(batch=16, s_max=1024, dtype=BF16):
+        """Llama-3-8B shape: 32 query heads over 8 KV heads (G = 4)."""
+        return LlamaConfig(layers=32, d_model=4096, heads=32, kv_heads=8, head_dim=128, ffn=14336, vocab=128256,
+                           s_max=s_max, batch=batch, dtype=dtype)
 
     @staticmethod
     def tiny(dtype=BF16, layers=2, batch=4):
@@ -73,20 +84,20 @@ class LlamaConfig:
                            batch=batch, dtype=dtype)
 
     def weight_elems(self, world: int = 1) -> int:
-        d, f = self.d_model, self.ffn
-        per_layer = (4 * d * d + 3 * d * f) // world + 2 * d
+        d, f, dkv = self.d_model, self.ffn, self.n_kv * self.head_dim
+        per_layer = (2 * d * d + 2 * d * dkv + 3 * d * f) // world + 2 * d
         return self.layers * per_layer + d + self.vocab * d + self.vocab * d  # + embedding table
 
     def algorithmic_bytes(self, pos: int, world: int = 1) -> int:
         """SURVEY.md 8(d): weights read once + KV read/append + ~12 activation tensors per layer."""
         e = 2 if self.dtype in (F16, BF16) else 4
-        d, f = self.d_model, self.ffn
-        proj = self.layers * ((4 * d * d + 3 * d * f) // world) + d * self.vocab
+        d, f, dkv = self.d_model, self.ffn, self.n_kv * self.head_dim
+        proj = self.layers * ((2 * d * d + 2 * d * dkv + 3 * d * f) // world) + d * self.vocab
         norms = self.layers * 2 * d + d
-        kv = self.layers * 2 * self.batch * (self.heads // world) * self.head_dim * (pos + 2)
+        kv = self.layers * 2 * self.batch * (self.n_kv // world) * self.head_dim * (pos + 2)
         act = self.layers * 12 * self.batch * d
         if self.fp8_weights:  # one byte per projection weight + 4 bytes per output column
-            cols = self.layers * ((3 * d + 2 * f) // world + 2 * d) + self.vocab
+            cols = self.layers * ((d + 2 * dkv + 2 * f) // world + 2 * d) + self.vocab
             return proj + 4 * cols + (norms + kv + act) * e
         return (proj + norms + kv + act) * e
 
@@ -105,10 +116,13 @@ class LlamaGraph:
 def build_llama_decode(h, cfg: LlamaConfig, world: int = 1, rank: int = 0) -> LlamaGraph:
     """One decode step.  world > 1 applies the reference's tensor-parallel cut (parallel_opt.py):
     q/k/v + gate/up column-split, o/down row-split followed by AllReduceSum, KV cache split by head,
-    embedding / norms / logits replicated."""
+    embedding / norms / logits replicated.  cfg.kv_heads < cfg.heads builds grouped-query attention: k / v projections
+    and caches carry the KV heads, query head i reads KV head i // (heads // kv_heads)."""
     assert cfg.heads % world == 0 and cfg.ffn % world == 0
+    assert cfg.n_kv % world == 0 and cfg.heads % cfg.n_kv == 0
     B, d, H, dh, f, V, dt = cfg.batch, cfg.d_model, cfg.heads // world, cfg.head_dim, cfg.ffn // world, cfg.vocab, cfg.dtype
-    dl = H * dh  # local attention width
+    Hkv = cfg.n_kv // world
+    dl, dkv = H * dh, Hkv * dh  # local attention widths of q and of k / v
     g = LlamaGraph(cfg)
 
     def weight(name, shape, kind, shard=None):
@@ -138,24 +152,24 @@ def build_llama_decode(h, cfg: LlamaConfig, world: int = 1, rank: int = 0) -> Ll
     x = h.gather(emb, g.input_ids, None, 0)  # [B,1,d]
     for li in range(cfg.layers):
         p = f"l{li}."
-        kc = h.tensor([B, H, cfg.s_max, dh], dt)
-        vc = h.tensor([B, H, cfg.s_max, dh], dt)
+        kc = h.tensor([B, Hkv, cfg.s_max, dh], dt)
+        vc = h.tensor([B, Hkv, cfg.s_max, dh], dt)
         kc.set_input()
         vc.set_input()
         g.k_caches.append(kc)
         g.v_caches.append(vc)
         hn = h.RMSNorm(x, weight(p + "ln1", (d,), "norm"), None)
         q = linear(hn, p + "wq", (d, dl), ("col", d))
-        k = linear(hn, p + "wk", (d, dl), ("col", d))
-        v = linear(hn, p + "wv", (d, dl), ("col", d))
+        k = linear(hn, p + "wk", (d, dkv), ("col", d))
+        v = linear(hn, p + "wv", (d, dkv), ("col", d))
         q = h.RoPE(g.position_ids, q, None)
         k = h.RoPE(g.position_ids, k, None)
 
-        def heads(t):
-            t = h.reshape(t, None, [B, 1, H, dh])
-            return h.transpose(t, None, [0, 2, 1, 3])  # [B,H,1,dh]
+        def heads(t, n=H):
+            t = h.reshape(t, None, [B, 1, n, dh])
+            return h.transpose(t, None, [0, 2, 1, 3])  # [B,n,1,dh]
 
-        attn = h.attentionKVCache(kc, vc, heads(q), heads(k), heads(v), g.position_ids, None)
+        attn = h.attentionKVCache(kc, vc, heads(q), heads(k, Hkv), heads(v, Hkv), g.position_ids, None)
         a = h.reshape(h.transpose(attn, None, [0, 2, 1, 3]), None, [B, 1, dl])
         o = linear(a, p + "wo", (dl, d), ("row", d))
         if world > 1:
@@ -242,8 +256,8 @@ def fill_llama_weights_host(g: LlamaGraph, world: int = 1, rank: int = 0, seed: 
 def llama_cache_values(cfg: LlamaConfig, layer: int, which: str, world: int = 1, rank: int = 0, seed: int = 2):
     """KV cache pre-filled with N(0,1)*0.5 (SURVEY 8(d)); full-head tensor then the rank's head slice."""
     rng = np.random.default_rng([seed, layer, 0 if which == "k" else 1])
-    full = rng.standard_normal((cfg.batch, cfg.heads, cfg.s_max, cfg.head_dim), dtype=np.float32) * np.float32(0.5)
-    hl = cfg.heads // world
+    full = rng.standard_normal((cfg.batch, cfg.n_kv, cfg.s_max, cfg.head_dim), dtype=np.float32) * np.float32(0.5)
+    hl = cfg.n_kv // world
     return np.ascontiguousarray(full[:, rank * hl:(rank + 1) * hl])
 
 

@@ -926,6 +926,10 @@ def parallel_model(model, world: int, rank: int, new_handler=None) -> Model:
     def last_axis(name):
         return len(shapes[name]) - 1
 
+    for nd in g.nodes:  # every rank needs whole KV heads (grouped-query attention may have fewer than `world`)
+        if nd.op_type == "AttentionKVCache" and nd.inputs[0] in inputs and inputs[nd.inputs[0]].dims[1] % world:
+            raise NotImplementedError(f"AttentionKVCache {nd.name}: {inputs[nd.inputs[0]].dims[1]} KV heads do not split "
+                                      f"over {world} ranks")
     unary_like = set(OnnxStub._UNARY) | {"Softmax", "Cast", "Dropout"}
     for idx, nd in enumerate(g.nodes):
         nd = Node(nd.op_type, list(nd.inputs), list(nd.outputs), nd.name, dict(nd.attrs))

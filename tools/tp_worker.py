@@ -48,7 +48,9 @@ def main():
     local = int(os.environ.get("LOCAL_RANK", rank))
     torch.cuda.set_device(local)
     dtype = int(os.environ.get("TP_DTYPE", "16"))
-    cfg = G.LlamaConfig(layers=2, d_model=1024, heads=8, head_dim=128, ffn=2816, vocab=2048, s_max=64, batch=16, dtype=dtype)
+    kv = os.environ.get("TP_KV_HEADS")  # grouped-query attention: KV heads of the unsharded model
+    cfg = G.LlamaConfig(layers=2, d_model=1024, heads=8, head_dim=128, ffn=2816, vocab=2048, s_max=64, batch=16, dtype=dtype,
+                        kv_heads=int(kv) if kv else None)
     out = os.environ["TP_OUT"]
     for mode in ("p2p", "nccl"):
         sched, logits = run(mode, cfg, rank, world, local)
