@@ -5,7 +5,8 @@ magnitude term is `S = |A64| @ |W64|`; a kernel that accumulates in fp32 and rou
 
     |got - ref| <= ulp_T(|ref|) + 2^-16 * S
 
-* ulp_T(x) = 2^(max(e, -126) - 7) for bf16 and 2^(max(e, -14) - 10) for fp16, e = floor(log2 |x|).  The one rounding to T is
+* ulp_T(x) = 2^(max(e, -126) - 7) for bf16, 2^(max(e, -14) - 10) for fp16 (and 2^(max(e, -126) - 23) for fp32, which
+  tests/attn64.py uses), e = floor(log2 |x|).  The one rounding to T is
   at most half an ulp; a sum that crosses a binade while it is rounded can double that, so one whole ulp of |ref| is allowed.
 * fp32 accumulation: the kernels add 16-product tensor-core partials into fp32 running sums of at most 11008 / 16 terms per
   split and then add at most 8 split partials.  Even if every one of those additions truncates, the running sums of products with
@@ -62,8 +63,7 @@ def product(a, w, block=4096):
 
 def ulp(x, dt):
     """ulp of the storage type at |x| (the ulp of its smallest normal below that, as for subnormals)"""
-    assert dt in (BF16, F16)
-    emin, mant = (-126, 7) if dt == BF16 else (-14, 10)
+    emin, mant = {BF16: (-126, 7), F16: (-14, 10), F32: (-126, 23)}[dt]
     ax = np.abs(np.asarray(x, np.float64))
     _, ex = np.frexp(ax)                  # ax = f * 2^ex with f in [0.5, 1): floor(log2 ax) = ex - 1
     e = np.where(ax > 0, ex - 1, emin)
