@@ -353,11 +353,13 @@ template <typename T, int D>
 static int launch_ap(const void *q, const void *k, const void *v, ApArgs a, cudaStream_t st, const ApStrides *sq = nullptr,
                      const ApStrides *sk = nullptr, const ApStrides *sv = nullptr) {
     CUtensorMap mq, mk, mv;
+    // Skv = 0 launches no K / V load (every row is written as 0), but a tensor map cannot have an empty dimension: one row
+    const int skv_map = a.Skv > 0 ? a.Skv : 1;
     if (!sq) {
         a.map_mode = 0;
         if (!make_tma_3d_b16(&mq, q, (uint64_t)a.BH, (uint64_t)a.Sq, (uint64_t)D, (uint64_t)D, (uint64_t)a.Sq * D, AP_BQ, 64) ||
-            !make_tma_3d_b16(&mk, k, (uint64_t)a.BH, (uint64_t)a.Skv, (uint64_t)D, (uint64_t)D, (uint64_t)a.Skv * D, AP_BK, 64) ||
-            !make_tma_3d_b16(&mv, v, (uint64_t)a.BH, (uint64_t)a.Skv, (uint64_t)D, (uint64_t)D, (uint64_t)a.Skv * D, 64, 64))
+            !make_tma_3d_b16(&mk, k, (uint64_t)a.BH, (uint64_t)skv_map, (uint64_t)D, (uint64_t)D, (uint64_t)skv_map * D, AP_BK, 64) ||
+            !make_tma_3d_b16(&mv, v, (uint64_t)a.BH, (uint64_t)skv_map, (uint64_t)D, (uint64_t)D, (uint64_t)skv_map * D, 64, 64))
             ITB_FAIL("attention_prefill: cuTensorMapEncodeTiled failed");
     } else {
         // 4-D maps, dimensions ordered by stride (TMA wants them ascending): (d, h, s, b) when heads are the inner stride (a fused
@@ -372,7 +374,7 @@ static int launch_ap(const void *q, const void *k, const void *v, ApArgs a, cuda
                            : make_tma_4d_b16(m, base, (uint64_t)D, (uint64_t)S, (uint64_t)a.H, (uint64_t)B, (uint64_t)t.s, (uint64_t)t.h,
                                              (uint64_t)t.b, 64, box_s, 1, 1);
         };
-        if (!mk4(&mq, q, *sq, a.Sq, AP_BQ) || !mk4(&mk, k, *sk, a.Skv, AP_BK) || !mk4(&mv, v, *sv, a.Skv, 64))
+        if (!mk4(&mq, q, *sq, a.Sq, AP_BQ) || !mk4(&mk, k, *sk, skv_map, AP_BK) || !mk4(&mv, v, *sv, skv_map, 64))
             ITB_FAIL("attention_prefill: cuTensorMapEncodeTiled (strided views) failed");
     }
     const int smem = 2 * AP_BQ * D * 2 + AP_BK * D * 2 + AP_BQ * AP_BK * 2 + AP_BK * AP_MPAD * 2 + AP_BK * AP_SLD * 2 + 1024;

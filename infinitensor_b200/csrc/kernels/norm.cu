@@ -277,7 +277,22 @@ static int launch_rowop(const char *name, const T *x, T *y, const T *scale, cons
     } else {
         int cache = dim <= 12288;
         int threads = dim >= 8192 ? 1024 : 512;
-        launch_k(row_block_kernel<T, MODE>, dim3((unsigned)outer), dim3(threads), cache ? dim * sizeof(float) : 0, st, x, y, scale, bias, dim, scale_size, bias_size, eps, cache);
+        const size_t smem = cache ? dim * sizeof(float) : 0;
+        // a cached row of up to 12288 floats fills the 48 KB a block gets without opting in, and the kernel's static reduction
+        // buffer comes on top: rows above 48 KB - 128 B need the larger dynamic limit (per device, once)
+        if (smem > 32 * 1024) {
+            static bool raised[64] = {false};
+            int dev = 0;
+            cudaGetDevice(&dev);
+            dev &= 63;
+            if (!raised[dev]) {
+                const cudaError_t e = cudaFuncSetAttribute(row_block_kernel<T, MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                                           12288 * (int)sizeof(float));
+                ITB_CHECK(e == cudaSuccess, "%s: smem attribute: %s", name, cudaGetErrorString(e));
+                raised[dev] = true;
+            }
+        }
+        launch_k(row_block_kernel<T, MODE>, dim3((unsigned)outer), dim3(threads), smem, st, x, y, scale, bias, dim, scale_size, bias_size, eps, cache);
     }
     ITB_LAUNCH_CHECK(name);
     return 0;
