@@ -1109,7 +1109,10 @@ static int64_t ds_scratch_bytes(int max_tiles, int max_slots, int BH, int S_max)
 
 extern "C" int64_t it_b200_decode_stack_workspace(int n_layers, int B, int d_model, int H, int S_max, int ffn) {
     (void)n_layers;
-    const int nctas = kNumSMs;
+    // the split factors, hence the partial slots, depend on the grid: size for the one the launch uses (one CTA per SM of the
+    // current device); kNumSMs only when no device answers
+    const int sms = ds_device_state().sms;
+    const int nctas = sms > 0 ? sms : kNumSMs;
     int max_tiles = 0, max_slots = 0;
     const int dl = H * DS_KD;
     const int shapes[4][3] = {{3, dl, d_model}, {1, d_model, dl}, {2, ffn, d_model}, {1, d_model, ffn}};  // groups, N, K

@@ -1,4 +1,4 @@
-"""GPU parity of the persistent decode kernel (decode_stack.cu) through the C-ABI: chains of tcgen05 skinny GEMM phases
+"""GPU parity of the persistent decode kernel (decode_stack.cu) through the C-ABI: chains of wgmma skinny GEMM phases
 with the RMSNorm / Silu*Mul operand transforms and the residual epilogue, and the whole decoder-layer stack, against the
 CPU oracle composed from the same operator sequence the graph executes (SURVEY 8(a) rows a1, a3, a6-a9).
 Tolerances: SURVEY 8(c) -- GEMM abs <= 2^-8 (bf16) / 2^-11 (fp16) * sqrt(K) * max|a| * max|b|, end-to-end rel-to-max."""
