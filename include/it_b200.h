@@ -266,7 +266,8 @@ int it_b200_conv2d_nhwc(int dtype, const void *x, const void *w, void *y, int y_
 
 /* ---- AttentionKVCache (decode, q-len 1): replaces _attention_kvcache_kernel_128_1/_2
  *      (attention_kvcache.cu:8-169).  Appends k,v IN PLACE into k_cache/v_cache at
- *      position_id[0]; caches [B,H,S_max,D], q/k/v/out [B,H,1,D]; D == 128.
+ *      position_id[0]; caches [B,H,S_max,D], q/k/v/out [B,H,1,D]; D == 128 (the reference's width, scale 1/sqrt(128))
+ *      or, as an extension for GPT-2 / TinyLlama-shape heads, D == 64; the scale is 1/sqrt(D).  Other D are refused.
  *      pos_dtype: ITB_I32 / ITB_U32 / ITB_I64 (element 0 is used for every row, .cu:17).
  *      Ordering contract (programmatic dependent launch): q / k / v (and the RoPE positions of the _rope variant) may come from
  *      the kernel launched just before on the same stream; `position_id` and the cache rows BELOW the position are read
@@ -299,8 +300,9 @@ int it_b200_allreduce_fused(int dtype, const void *in, const void *residual, con
                             int *timeout_flag, void *stream);
 
 /* ---- AttentionKVCache with the layer's two RoPE ops folded in: q_pre / k_pre are the PRE-RoPE projections
- *      ([B, H*128] == [B,H,1,128]); RoPE (rotate-half, dim_head 128, position rope_pos[b]) is applied on load, the
- *      rotated k is what gets appended -- bit-identical to RoPE -> AttentionKVCache (rope.cu:7-31 + attention_kvcache.cu). ---- */
+ *      ([B, H*D] == [B,H,1,D], D = 128 or 64); RoPE (rotate-half over each D-wide head, i.e. it_b200_rope with dim_head = D,
+ *      position rope_pos[b]) is applied on load, the rotated k is what gets appended -- bit-identical to RoPE ->
+ *      AttentionKVCache (rope.cu:7-31 + attention_kvcache.cu). ---- */
 int it_b200_attention_kvcache_rope(int dtype, void *k_cache, void *v_cache, const void *q_pre, const void *k_pre,
                                    const void *v, const void *position_id, int pos_dtype, const void *rope_pos,
                                    int rope_pos_dtype, void *out, int B, int H, int S_max, int D, void *workspace,

@@ -307,6 +307,8 @@ def _ids(ts):
 class GraphHandler:
     """reference GraphHandlerObj (include/core/graph_handler.h:15-159) as bound at ffi_infinitensor.cc:548-638."""
 
+    head_widths = (64, 128)  # decode attention / RoPE head widths (64: extension; the reference's are 128)
+
     def __init__(self, runtime: CudaRuntime):
         if not isinstance(runtime, CudaRuntime):
             raise RuntimeError("GraphHandler needs a backend.CudaRuntime")
@@ -427,8 +429,9 @@ class GraphHandler:
         return self._op1("AttentionKVCache", [input_k_cache, input_v_cache, input_q, input_k, input_v, position_id],
                          output_matmul, [1] if per_row_positions else [])
 
-    def RoPE(self, pos, input, output):
-        return self._op1("RoPE", [pos, input], output)
+    def RoPE(self, pos, input, output, dim_head=128):
+        """dim_head (extension): rotate-half within heads of this width; the reference fixes it at 128 (rope.cc:25)."""
+        return self._op1("RoPE", [pos, input], output, [] if dim_head == 128 else [int(dim_head)])
 
     def split(self, input, outputs, axis, numOrRatio):
         if isinstance(numOrRatio, int):

@@ -202,7 +202,11 @@ class RoPEB200 : public CudaKernelWithoutConfig {
         const auto &d = x->getDims();
         IT_ASSERT(d.size() == 3 && pos->getRank() == 2, "RoPE: input [B,S,dim_model], pos [B,S]");
         IT_ASSERT(d[0] == pos->getDims()[0] && d[1] == pos->getDims()[1], "RoPE: pos / input mismatch");
+#ifdef ITB_SEAM_A
         const int dim_head = 128;  // hard-coded in the reference (rope.cc:25)
+#else
+        const int dim_head = as<RoPEObj>(op)->getDimHead();  // extension: 128 unless the graph gave another width
+#endif
         CK(it_b200_rope(DTI(x), P(pos), DTI(pos), P(x), P(op->getOutput()), d[0], d[1], d[2], dim_head, S()), op);
     }
 };

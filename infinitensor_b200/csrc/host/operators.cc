@@ -122,8 +122,9 @@ RMSNormObj::RMSNormObj(GraphObj *graph, Tensor input, Tensor weight, Tensor outp
     IT_ASSERT(checkValid(graph));
 }
 
-RoPEObj::RoPEObj(GraphObj *graph, Tensor pos, Tensor input, Tensor output)
-    : OperatorObj(OpType::RoPE, {pos, input}, {output}) {
+RoPEObj::RoPEObj(GraphObj *graph, Tensor pos, Tensor input, Tensor output, int dimHead)
+    : OperatorObj(OpType::RoPE, {pos, input}, {output}), dimHead(dimHead) {
+    IT_ASSERT(dimHead > 0 && dimHead % 2 == 0, "RoPE: dim_head " + std::to_string(dimHead) + " must be positive and even");
     IT_ASSERT(checkValid(graph));
 }
 

@@ -107,8 +107,12 @@ class RMSNormObj : public OperatorObj {
 };
 
 class RoPEObj : public OperatorObj {
+    int dimHead;  // extension: rotate-half over heads of this width; the reference fixes it at 128 (rope.cc:25)
+
   public:
-    RoPEObj(GraphObj *graph, Tensor pos, Tensor input, Tensor output);
+    RoPEObj(GraphObj *graph, Tensor pos, Tensor input, Tensor output, int dimHead = 128);
+    int getDimHead() const { return dimHead; }
+    vector<int> getOpAttrVector() const override { return {(int)type.underlying(), dimHead}; }
     std::optional<vector<Shape>> inferShape(const TensorVec &inputs) override { return {{inputs[1]->getDims()}}; }
     vector<DataType> inferDataType(const TensorVec &ins) const override { return {ins[1]->getDType()}; }
 };

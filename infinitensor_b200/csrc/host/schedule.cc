@@ -659,18 +659,20 @@ const vector<ExecStep> &GraphObj::getSchedule() {
                 }
             }
         } else if (type == OpType::RoPE && (mask & 32)) {
-            // RoPE -> (alias-only chain) -> AttentionKVCache q / k operand, S = 1, 128-wide heads: fold into the attention kernel
+            // RoPE -> (alias-only chain) -> AttentionKVCache q / k operand, S = 1, heads of the RoPE's width D in {64, 128}:
+            // fold into the attention kernel.  A RoPE whose width is not the cache's head width runs unfused.
+            const int dh = as<RoPEObj>(op)->getDimHead();
             Tensor t = op->getOutput();
             bool chain = !t->isOutput();
             while (chain && t->getTargets().size() == 1 && (mask & 1) && aliasable(t->getTargets()[0])) t = t->getTargets()[0]->getOutput();
             auto &xd = op->getInputs(1)->getDims();
             if (chain && t->getTargets().size() == 1 && t->getTargets()[0]->getOpType() == OpType::AttentionKVCache &&
-                xd.size() == 3 && xd[1] == 1 && xd[2] % 128 == 0 && op->getInputs(1)->getDType().isFloat()) {
+                (dh == 64 || dh == 128) && xd.size() == 3 && xd[1] == 1 && xd[2] % dh == 0 && op->getInputs(1)->getDType().isFloat()) {
                 auto att = t->getTargets()[0];
                 // the operand this RoPE feeds: q carries Hq heads, k the caches' Hkv (fewer under grouped-query attention)
                 auto &qd = (att->getInputs(2) == t ? att->getInputs(2) : att->getInputs(3))->getDims();
-                if ((att->getInputs(2) == t || att->getInputs(3) == t) && qd[2] == 1 && qd[3] == 128 && qd[0] == xd[0] &&
-                    qd[1] * 128 == xd[2]) {
+                if ((att->getInputs(2) == t || att->getInputs(3) == t) && qd[2] == 1 && qd[3] == dh && qd[0] == xd[0] &&
+                    qd[1] * dh == xd[2]) {
                     deferredInto[att.get()].push_back(op);
                     deferred.insert(op.get());
                     continue;

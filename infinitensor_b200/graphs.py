@@ -1,13 +1,17 @@
 """Synthetic graph builders for the BASELINE.json configs, written against the GraphHandler API only
 (the same calls OnnxStub makes, reference pyinfinitensor/src/pyinfinitensor/onnx.py:136-1117), so they
 need no `onnx` package.  Every builder takes a duck-typed handler: `backend.GraphHandler` (the product)
-or `oracle.graph_oracle.OracleHandler` (the CPU checker) -- one graph description, two executors.
+or `oracle.graph_oracle.OracleHandler` (the CPU checker) -- one graph description, two executors.  Decode graphs with
+attention heads narrower than 128 (GPT-2, TinyLlama) use an extension of the reference, whose AttentionKVCache scale and
+RoPE are fixed at 128: they build only on a handler that lists the width in its `head_widths` (`GraphHandler` does;
+`OracleHandler`, which restates the reference, does not), so no executor quietly applies the 128-wide rule to them.
 
   build_llama_decode   -- config C3/C5: Llama-7B-shape KV-cache decode step (op mix of
                           examples/python/llama_kvcache_inference.py:45-80 with fused RMSNorm / RoPE /
                           AttentionKVCache nodes), optionally tensor-parallel-sharded exactly where
                           examples/distributed/parallel_opt.py:9-247 cuts the graph.
   build_gpt2           -- config C2: GPT-2-small forward, B=1 S=128 (op mix of run_pytorch.py:89-108 export)
+  build_gpt2_decode    -- one GPT-2 KV-cache decode step over the same weights (64-wide heads)
   build_resnet50       -- config C4: ResNet-50 forward (conv + BN + relu + pooling + fc)
   build_matmul         -- config C1: single MatMul
 """
@@ -53,6 +57,11 @@ def from_storage(a: np.ndarray, dtype: int) -> np.ndarray:
     return a
 
 
+def _require_head_width(h, dh: int):
+    if dh != 128 and dh not in getattr(h, "head_widths", (128,)):
+        raise NotImplementedError(f"{type(h).__name__} does not execute {dh}-wide attention heads (the reference's are 128-wide)")
+
+
 # ---------------------------------------------------------------- Llama decode (C3 / C5)
 @dataclass
 class LlamaConfig:
@@ -82,6 +91,12 @@ class LlamaConfig:
     def tiny(dtype=BF16, layers=2, batch=4):
         return LlamaConfig(layers=layers, d_model=256, heads=2, head_dim=128, ffn=512, vocab=1000, s_max=64,
                            batch=batch, dtype=dtype)
+
+    @staticmethod
+    def tinyllama_1b(batch=16, s_max=1024, dtype=BF16, layers=22):
+        """TinyLlama-1.1B shape: 32 query heads of 64 over 4 KV heads (G = 8)."""
+        return LlamaConfig(layers=layers, d_model=2048, heads=32, kv_heads=4, head_dim=64, ffn=5632, vocab=32000,
+                           s_max=s_max, batch=batch, dtype=dtype)
 
     def weight_elems(self, world: int = 1) -> int:
         d, f, dkv = self.d_model, self.ffn, self.n_kv * self.head_dim
@@ -123,6 +138,8 @@ def build_llama_decode(h, cfg: LlamaConfig, world: int = 1, rank: int = 0) -> Ll
     B, d, H, dh, f, V, dt = cfg.batch, cfg.d_model, cfg.heads // world, cfg.head_dim, cfg.ffn // world, cfg.vocab, cfg.dtype
     Hkv = cfg.n_kv // world
     dl, dkv = H * dh, Hkv * dh  # local attention widths of q and of k / v
+    _require_head_width(h, dh)
+    rope_kw = {} if dh == 128 else {"dim_head": dh}  # 128-wide graphs make the reference's RoPE call
     g = LlamaGraph(cfg)
 
     def weight(name, shape, kind, shard=None):
@@ -162,8 +179,8 @@ def build_llama_decode(h, cfg: LlamaConfig, world: int = 1, rank: int = 0) -> Ll
         q = linear(hn, p + "wq", (d, dl), ("col", d))
         k = linear(hn, p + "wk", (d, dkv), ("col", d))
         v = linear(hn, p + "wv", (d, dkv), ("col", d))
-        q = h.RoPE(g.position_ids, q, None)
-        k = h.RoPE(g.position_ids, k, None)
+        q = h.RoPE(g.position_ids, q, None, **rope_kw)
+        k = h.RoPE(g.position_ids, k, None, **rope_kw)
 
         def heads(t, n=H):
             t = h.reshape(t, None, [B, 1, n, dh])
@@ -290,6 +307,18 @@ class GPT2Config:
     def tiny(dtype=F16):
         return GPT2Config(layers=2, d_model=64, heads=2, ffn=128, vocab=500, n_pos=64, seq=16, batch=1, dtype=dtype)
 
+    def algorithmic_bytes(self, pos: int) -> int:
+        """One decode step (build_gpt2_decode) at position `pos`, as LlamaConfig.algorithmic_bytes counts it: every layer's
+        weights and biases read once, the KV cache read and appended, ~12 activation tensors per layer, the two embedding
+        rows per batch row, and the tied logits head (the whole embedding table) when there is one."""
+        e = 2 if self.dtype in (F16, BF16) else 4
+        B, d, f = self.batch, self.d_model, self.ffn
+        per_layer = 3 * d * d + 3 * d + d * d + d + 2 * d * f + f + d + 4 * d
+        weights = self.layers * per_layer + 2 * d + 2 * B * d + (self.vocab * d if self.lm_head else 0)
+        kv = self.layers * 2 * B * d * (pos + 2)
+        act = self.layers * 12 * B * d
+        return (weights + kv + act) * e
+
 
 @dataclass
 class GPT2Graph:
@@ -299,6 +328,8 @@ class GPT2Graph:
     out: object = None
     weights: dict = field(default_factory=dict)
     consts: dict = field(default_factory=dict)  # name -> (tensor, float32 ndarray)
+    k_caches: list = field(default_factory=list)  # build_gpt2_decode: per layer [B, H, s_max, dh]
+    v_caches: list = field(default_factory=list)
 
 
 def build_gpt2(h, cfg: GPT2Config) -> GPT2Graph:
@@ -352,6 +383,62 @@ def build_gpt2(h, cfg: GPT2Config) -> GPT2Graph:
         m = h.matmul(m, weight(p + "fc2.w", (f, d), "proj"), None, False, False, weight(p + "fc2.b", (d,), "bias"), LINEAR)
         x = h.add(x, m, None)
     x = h.layerNormalization(x, weight("ln_f.w", (d,), "norm"), None, weight("ln_f.b", (d,), "bias"), 1e-5, -1, 1)
+    if cfg.lm_head:
+        x = h.matmul(x, g.weights["wte"][0], None, False, True, None, LINEAR)  # tied embedding
+    g.out = x
+    g.out.set_output()
+    return g
+
+
+def build_gpt2_decode(h, cfg: GPT2Config, s_max: int) -> GPT2Graph:
+    """One KV-cache decode step of build_gpt2's model: input_ids / position_ids [B, 1] (position_ids[0] is every row's
+    position, the AttentionKVCache rule), per layer LayerNorm, c_attn + bias split into q / k / v heads [B, H, 1, dh],
+    AttentionKVCache over caches [B, H, s_max, dh] (graph inputs, appended in place), merge, proj + bias, residual, LayerNorm,
+    fc + bias, Gelu, fc2 + bias, residual; the final LayerNorm and (cfg.lm_head) the tied-embedding logits.  Same weight
+    names and shapes as build_gpt2, so fill_gpt2_weights_host fills either; the caches are in `k_caches` / `v_caches`."""
+    B, d, H, f, dt = cfg.batch, cfg.d_model, cfg.heads, cfg.ffn, cfg.dtype
+    dh = d // H
+    _require_head_width(h, dh)
+    g = GPT2Graph(cfg)
+
+    def weight(name, shape, kind):
+        t = h.tensor(list(shape), dt)
+        t.set_weight()
+        g.weights[name] = (t, tuple(shape), kind, None)
+        return t
+
+    def linear(x_, name, k, n):
+        return h.matmul(x_, weight(name + ".w", (k, n), "proj"), None, False, False, weight(name + ".b", (n,), "bias"), LINEAR)
+
+    def layer_norm(x_, name):
+        return h.layerNormalization(x_, weight(name + ".w", (d,), "norm"), None, weight(name + ".b", (d,), "bias"), 1e-5, -1, 1)
+
+    g.input_ids = h.tensor([B, 1], I64)
+    g.position_ids = h.tensor([B, 1], I64)
+    g.input_ids.set_input()
+    g.position_ids.set_input()
+    x = h.add(h.gather(weight("wte", (cfg.vocab, d), "embed"), g.input_ids, None, 0),
+              h.gather(weight("wpe", (cfg.n_pos, d), "embed"), g.position_ids, None, 0), None)  # [B,1,d]
+    for li in range(cfg.layers):
+        p = f"h{li}."
+        kc = h.tensor([B, H, s_max, dh], dt)
+        vc = h.tensor([B, H, s_max, dh], dt)
+        kc.set_input()
+        vc.set_input()
+        g.k_caches.append(kc)
+        g.v_caches.append(vc)
+        qkv = linear(layer_norm(x, p + "ln1"), p + "attn", d, 3 * d)
+        q, k, v = h.split(qkv, None, 2, 3)
+
+        def heads(t):
+            return h.transpose(h.reshape(t, None, [B, 1, H, dh]), None, [0, 2, 1, 3])  # [B,H,1,dh]
+
+        a = h.attentionKVCache(kc, vc, heads(q), heads(k), heads(v), g.position_ids, None)
+        a = h.reshape(h.transpose(a, None, [0, 2, 1, 3]), None, [B, 1, d])
+        x = h.add(x, linear(a, p + "proj", d, d), None)
+        m = h.gelu(linear(layer_norm(x, p + "ln2"), p + "fc", d, f), None)
+        x = h.add(x, linear(m, p + "fc2", f, d), None)
+    x = layer_norm(x, "ln_f")
     if cfg.lm_head:
         x = h.matmul(x, g.weights["wte"][0], None, False, True, None, LINEAR)  # tied embedding
     g.out = x

@@ -542,8 +542,13 @@ class OnnxStub:
                                            a.get("stash_type", 1))
         elif op == "RMSNorm":
             T[out0] = h.RMSNorm(I(0), I(1), None)
-        elif op == "RoPE":
-            T[out0] = h.RoPE(I(0), I(1), None)
+        elif op == "RoPE":  # optional int attribute dim_head (extension; absent = the reference's 128)
+            if "dim_head" in a and int(a["dim_head"]) != 128:
+                if int(a["dim_head"]) not in getattr(h, "head_widths", (128,)):
+                    raise NotImplementedError(f"RoPE {nd.name}: {type(h).__name__} does not execute dim_head {a['dim_head']}")
+                T[out0] = h.RoPE(I(0), I(1), None, int(a["dim_head"]))
+            else:
+                T[out0] = h.RoPE(I(0), I(1), None)
         elif op == "AttentionKVCache":
             T[out0] = h.attentionKVCache(I(0), I(1), I(2), I(3), I(4), I(5), None)
         elif op in ("MaxPool", "AveragePool"):
@@ -740,7 +745,10 @@ class OnnxExporter:
                           {"epsilon": float(eps), "axis": int(axis), "stash_type": int(stash_type)})
 
     def RMSNorm(self, x, w, y): return self._emit("RMSNorm", [x, w], self.inner.RMSNorm(x.inner, w.inner, self._in(y)))
-    def RoPE(self, pos, x, y): return self._emit("RoPE", [pos, x], self.inner.RoPE(pos.inner, x.inner, self._in(y)))
+    def RoPE(self, pos, x, y, dim_head=128):  # the attribute only when it is not the reference's 128: older files stay as they were
+        extra = [] if dim_head == 128 else [int(dim_head)]
+        return self._emit("RoPE", [pos, x], self.inner.RoPE(pos.inner, x.inner, self._in(y), *extra),
+                          {"dim_head": extra[0]} if extra else None)
 
     def attentionKVCache(self, kc, vc, q, k, v, pos, y):
         r = self.inner.attentionKVCache(kc.inner, vc.inner, q.inner, k.inner, v.inner, pos.inner, self._in(y))

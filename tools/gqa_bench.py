@@ -1,12 +1,15 @@
 #!/usr/bin/env python
 """Grouped-query decode attention on the GPU: kernel timing over KV head counts, and a Llama-3-8B-shape decode step.
 
-  python tools/gqa_bench.py [--iters 100] [--steps 50] [--warmup 10] [--no-step]
+  python tools/gqa_bench.py [--iters 100] [--steps 50] [--warmup 10] [--no-step] [--head-dim {64,128}]
+                            [--model {llama3_8b,tinyllama_1b}]
 
-Kernel: B 16, Hq 32, Hkv in {32, 8, 4, 1}, (S_max, p) in {(1024, 511), (4096, 4095)}, bf16, RoPE folded off.  Launches are
-timed with CUDA events and rotate over enough cache buffers (>= 6, >= 256 MB in all) that the caches are not L2-resident.
-Algorithmic bytes: the K and V rows read (B Hkv 2 p 128 e), the appended rows (B Hkv 2 128 e) and q / out (B Hq 2 128 e).
-Step: LlamaConfig.llama3_8b() at p 511, CUDA-graph replay; the roofline is graphs.LlamaConfig.algorithmic_bytes over the
+Kernel: B 16, Hq 32, Hkv in {32, 8, 4, 1}, (S_max, p) in {(1024, 511), (4096, 4095)}, bf16, head width --head-dim, RoPE
+folded off.  Launches are timed with CUDA events and rotate over enough cache buffers (>= 6, >= 256 MB in all) that the caches
+are not L2-resident.  Algorithmic bytes: the K and V rows read (B Hkv 2 p D e), the appended rows (B Hkv 2 D e) and q / out
+(B Hq 2 D e).  At --head-dim 64 the run also times, back to back, the streaming kernel at B 16, H 64, D 64 and at B 16, H 32,
+D 128 (S_max 4096, p 4095): the same bytes, so the GB/s ratio is what the narrower rows cost.
+Step: LlamaConfig.<model>() at p 511, CUDA-graph replay; the roofline is graphs.LlamaConfig.algorithmic_bytes over the
 H100 SXM data-sheet 3.35 TB/s -- a bound computed from the shapes, not a measurement.  The card's name, power limit and
 SM clock are printed from the same run."""
 import argparse
@@ -33,29 +36,29 @@ def card():
         return "nvidia-smi unavailable"
 
 
-def kernel_bytes(B, Hq, Hkv, p, e=2):
-    return B * Hkv * 2 * p * 128 * e + B * Hkv * 2 * 128 * e + B * Hq * 2 * 128 * e
+def kernel_bytes(B, Hq, Hkv, p, e=2, D=128):
+    return B * Hkv * 2 * p * D * e + B * Hkv * 2 * D * e + B * Hq * 2 * D * e
 
 
-def time_kernel(B, Hq, Hkv, S, p, iters):
+def time_kernel(B, Hq, Hkv, S, p, iters, D=128):
     st = ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
-    set_bytes = 2 * B * Hkv * S * 128 * 2
+    set_bytes = 2 * B * Hkv * S * D * 2
     nbuf = max(6, -(-(256 << 20) // set_bytes))
-    caches = [(torch.randn(B, Hkv, S, 128, device="cuda").bfloat16(), torch.randn(B, Hkv, S, 128, device="cuda").bfloat16())
+    caches = [(torch.randn(B, Hkv, S, D, device="cuda").bfloat16(), torch.randn(B, Hkv, S, D, device="cuda").bfloat16())
               for _ in range(nbuf)]
-    q = torch.randn(B, Hq, 1, 128, device="cuda").bfloat16()
-    k = torch.randn(B, Hkv, 1, 128, device="cuda").bfloat16()
-    v = torch.randn(B, Hkv, 1, 128, device="cuda").bfloat16()
+    q = torch.randn(B, Hq, 1, D, device="cuda").bfloat16()
+    k = torch.randn(B, Hkv, 1, D, device="cuda").bfloat16()
+    v = torch.randn(B, Hkv, 1, D, device="cuda").bfloat16()
     out = torch.empty_like(q)
     pos = torch.tensor([p], dtype=torch.int64, device="cuda")
-    wsb = L.lib.it_b200_attention_kvcache_workspace(B, Hq, S, 128)
+    wsb = L.lib.it_b200_attention_kvcache_workspace(B, Hq, S, D)
     ws = torch.empty(max(int(wsb), 16), dtype=torch.uint8, device="cuda")
     P = lambda t: ctypes.c_void_p(t.data_ptr())
 
     def launch(i):
         kc, vc = caches[i % nbuf]
         L.check(L.lib.it_b200_attention_kvcache_gqa(BF16, P(kc), P(vc), P(q), P(k), P(v), P(pos), 7, None, 7, P(out), B, Hq,
-                                                    Hkv, S, 128, P(ws), int(wsb), st))
+                                                    Hkv, S, D, P(ws), int(wsb), st))
 
     for i in range(2 * nbuf):
         launch(i)
@@ -72,10 +75,10 @@ def time_kernel(B, Hq, Hkv, S, p, iters):
     return us, nbuf
 
 
-def time_step(steps, warmup, pos=511):
+def time_step(steps, warmup, pos=511, model="llama3_8b"):
     from infinitensor_b200 import backend as B
     from infinitensor_b200 import graphs as G
-    cfg = G.LlamaConfig.llama3_8b()
+    cfg = getattr(G.LlamaConfig, model)()
     rt = B.CudaRuntime(0)
     h = B.GraphHandler(rt)
     g = G.build_llama_decode(h, cfg)
@@ -118,24 +121,36 @@ def main():
     ap.add_argument("--steps", type=int, default=50)
     ap.add_argument("--warmup", type=int, default=10)
     ap.add_argument("--no-step", action="store_true")
+    ap.add_argument("--head-dim", type=int, choices=(64, 128), default=128)
+    ap.add_argument("--model", choices=("llama3_8b", "tinyllama_1b"), default="llama3_8b")
     a = ap.parse_args()
     assert torch.cuda.is_available(), "gqa_bench needs a GPU"
+    D = a.head_dim
     print(f"card: {card()}")
-    print(f"{'B':>3} {'Hq':>3} {'Hkv':>3} {'S_max':>5} {'p':>5} {'bufs':>4} {'us':>9} {'MB':>9} {'GB/s':>8} {'of 3.35TB/s':>11}")
+    print(f"{'B':>3} {'Hq':>3} {'Hkv':>3} {'D':>3} {'S_max':>5} {'p':>5} {'bufs':>4} {'us':>9} {'MB':>9} {'GB/s':>8} "
+          f"{'of 3.35TB/s':>11}")
     res = {}
+
+    def row(B, Hq, Hkv, S, p, d):
+        us, nbuf = time_kernel(B, Hq, Hkv, S, p, a.iters, d)
+        byts = kernel_bytes(B, Hq, Hkv, p, D=d)
+        gbs = byts / us / 1e3
+        print(f"{B:>3} {Hq:>3} {Hkv:>3} {d:>3} {S:>5} {p:>5} {nbuf:>4} {us:>9.2f} {byts / 1e6:>9.2f} {gbs:>8.1f} "
+              f"{gbs * 1e9 / HBM:>10.1%}")
+        return us, gbs
+
     for S, p in ((1024, 511), (4096, 4095)):
         for Hkv in (32, 8, 4, 1):
-            us, nbuf = time_kernel(16, 32, Hkv, S, p, a.iters)
-            byts = kernel_bytes(16, 32, Hkv, p)
-            gbs = byts / us / 1e3
-            res[(S, Hkv)] = (us, gbs)
-            print(f"{16:>3} {32:>3} {Hkv:>3} {S:>5} {p:>5} {nbuf:>4} {us:>9.2f} {byts / 1e6:>9.2f} {gbs:>8.1f} "
-                  f"{gbs * 1e9 / HBM:>10.1%}")
+            res[(S, Hkv)] = row(16, 32, Hkv, S, p, D)
     print(f"p 511: Hkv 8 / Hkv 32 time = {res[(1024, 8)][0] / res[(1024, 32)][0]:.3f}; "
           f"p 4095: Hkv 8 / Hkv 32 GB/s = {res[(4096, 8)][1] / res[(4096, 32)][1]:.3f}")
+    if D == 64:
+        narrow, wide = row(16, 64, 64, 4096, 4095, 64), row(16, 32, 32, 4096, 4095, 128)
+        print(f"same bytes, D 64 (H 64) / D 128 (H 32) GB/s = {narrow[1] / wide[1]:.3f}")
     if not a.no_step:
-        cfg, ms, byts, sched = time_step(a.steps, a.warmup)
-        print(f"llama3_8b step (B {cfg.batch}, p 511, {cfg.layers} layers, {cfg.heads} q / {cfg.kv_heads} kv heads, bf16, "
+        cfg, ms, byts, sched = time_step(a.steps, a.warmup, model=a.model)
+        print(f"{a.model} step (B {cfg.batch}, p 511, {cfg.layers} layers, {cfg.heads} q / {cfg.n_kv} kv heads of "
+              f"{cfg.head_dim}, bf16, "
               f"CUDA graph, {a.steps} steps): {ms:.3f} ms/step, {cfg.batch / ms * 1e3:.0f} tok/s; algorithmic bytes "
               f"{byts / 1e9:.2f} GB -> bound {byts / HBM * 1e3:.2f} ms at 3.35 TB/s = {byts / HBM * 1e3 / ms:.1%} of roofline; "
               f"{sum(s.startswith('AttentionRope') for s in sched)} AttentionRope steps")

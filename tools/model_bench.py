@@ -1,7 +1,9 @@
 #!/usr/bin/env python
 """Whole-graph timings of the two non-headline BASELINE configs (parity-test cases, not bench lines):
-   C2 GPT-2-small (B=1, S=128, fp16) and C4 ResNet-50 (B=64, fp16), CUDA-graph replay, device-timed.
-   python tools/model_bench.py [gpt2] [resnet] [--batch N]"""
+   C2 GPT-2-small (B=1, S=128, fp16) and C4 ResNet-50 (B=64, fp16), CUDA-graph replay, device-timed;
+   gpt2-decode: one GPT-2-small KV-cache decode step (B 16, p 511, fp16, with the tied LM head), ms / step and its share of
+   the GPT2Config.algorithmic_bytes bound at the HBM peak.  The card's name, power limit and SM clock are printed with each.
+   python tools/model_bench.py [gpt2] [gpt2-decode] [resnet] [--batch N]"""
 import json
 import os
 import sys
@@ -11,6 +13,7 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np
 import torch
 
+from gqa_bench import card  # noqa: E402 (tools/ is this script's directory)
 from infinitensor_b200 import backend as B, graphs as G
 
 _PEAKS_PATH = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "MEASURED_PEAKS.json")
@@ -57,6 +60,27 @@ def gpt2():
                       "weight_bytes": wbytes, "hbm_floor_ms": round(wbytes / PEAKS["hbm_gbs"] / 1e6, 4)}))
 
 
+def gpt2_decode(batch=16, pos=511):
+    cfg = G.GPT2Config(batch=batch, lm_head=True)
+    rt = B.CudaRuntime(0)
+    h = B.GraphHandler(rt)
+    g = G.build_gpt2_decode(h, cfg, 1024)
+    h.data_malloc()
+    G.fill_gpt2_weights_host(g)
+    rng = np.random.default_rng(2)
+    for c in g.k_caches + g.v_caches:
+        c.copyin_numpy((rng.standard_normal(c.shape(), dtype=np.float32) * 0.5).astype(np.float16))
+    g.input_ids.copyin_numpy(rng.integers(0, cfg.vocab, size=(batch, 1)).astype(np.int64))
+    g.position_ids.copyin_numpy(np.full((batch, 1), pos, np.int64))
+    ms, launches = timed(h, rt, 100)
+    byts = cfg.algorithmic_bytes(pos)
+    floor = byts / PEAKS["hbm_gbs"] / 1e6
+    print(json.dumps({"config": f"gpt2-small decode step B={batch} p={pos} fp16 (tied LM head)", "ms_per_step": round(ms, 4),
+                      "tokens_per_s": round(batch / ms * 1e3, 1), "algorithmic_bytes": byts, "hbm_floor_ms": round(floor, 4),
+                      "frac_of_bound": round(floor / ms, 4), "launches_per_step": launches,
+                      "scheduled_steps": len(h.schedule()), "card": card()}))
+
+
 def resnet(batch):
     cfg = G.ResNetConfig(batch=batch)
     rt = B.CudaRuntime(0)
@@ -83,5 +107,7 @@ if __name__ == "__main__":
         batch = int(sys.argv[sys.argv.index("--batch") + 1])
     if "gpt2" in args:
         gpt2()
+    if "gpt2-decode" in args:
+        gpt2_decode()
     if "resnet" in args:
         resnet(batch)
