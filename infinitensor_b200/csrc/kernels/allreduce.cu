@@ -77,9 +77,11 @@ __global__ void __launch_bounds__(512) allreduce_ll_kernel(ArPeers peers, int wo
     int *epoch_p = (int *)(local + ar_epoch_off()) + row;
     const int nv = hidden / V;
     pdl_wait();  // `in` comes from the preceding row-split MatMul; epoch[row] from the previous all-reduce kernel
-    const int e = *epoch_p;  // only CTA `row` of this stream's kernels ever writes epoch[row]
+    // only CTA `row` of this stream's kernels ever writes epoch[row]; unsigned, so that the count wraps past INT_MAX (2^31
+    // all-reduces of one row) without signed overflow: tag and parity follow the bits through the wrap
+    const uint32_t e = (uint32_t)*epoch_p;
     const int b = e & 1;
-    const uint32_t tag = (uint32_t)(e + 1);
+    const uint32_t tag = e + 1u;
     bool gave_up = false;
     const size_t slot = (((size_t)b * AR_MAX_WORLD + rank) * AR_MAX_ROWS + row) * AR_SLOT_BYTES;
 
@@ -149,7 +151,7 @@ __global__ void __launch_bounds__(512) allreduce_ll_kernel(ArPeers peers, int wo
         }
     }
     __syncthreads();
-    if (threadIdx.x == 0) *epoch_p = e + 1;
+    if (threadIdx.x == 0) *epoch_p = (int)(e + 1u);
 }
 
 }  // namespace itb
