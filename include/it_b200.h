@@ -338,44 +338,6 @@ int it_b200_attention_prefill_strided(int dtype, const void *q, const void *k, c
                                       const void *mask, int64_t mask_stride_b, int64_t mask_stride_h, int64_t mask_stride_i,
                                       int64_t mask_stride_j, void *stream);
 
-/* ---- The persistent decode kernel (decode_stack.cu): a whole stack of Llama decoder layers in ONE launch.
- *      Per layer it replaces the eight launches of the fused schedule -- RMSNorm (rms_norm.cu:36-110), the q/k/v MatMuls
- *      (matmul.cc:66-211), RoPE x2 (rope.cu:7-88) + AttentionKVCache (attention_kvcache.cu:8-169), the o-proj MatMul + Add
- *      (element_wise.cc), RMSNorm, the gate/up MatMuls, Silu (unary.cu:123) * Mul, the down MatMul + Add -- with five
- *      phases of one persistent grid separated by a grid barrier; every intermediate tensor of the operator graph is still
- *      written (q, k, v, attn_out, x_mid, gate, up, x_out: [B, width] row-major, same dtype) with the rounding the separate
- *      kernels apply.  B <= 16 rows; head dim 128; weights [K, N] row-major as ONNX MatMul stores them.
- *      pos_flags / rope_pos as for it_b200_attention_kvcache_rope (rope_pos NULL: no RoPE). ---- */
-typedef struct {
-    const void *ln1_w, *wq, *wk, *wv, *wo, *ln2_w, *wg, *wu, *wd; /* weights */
-    void *k_cache, *v_cache;                                      /* [B, H, S_max, 128], appended in place */
-    void *q, *k, *v;                                              /* [B, H*128] projections (q, k before RoPE) */
-    void *attn_out;                                               /* [B, H*128] */
-    void *x_mid;                                                  /* [B, d_model] = x + attn_out . wo */
-    void *gate, *up;                                              /* [B, ffn] */
-    void *x_out;                                                  /* [B, d_model] = x_mid + (silu(gate) * up) . wd */
-} itb_llama_layer;
-int64_t it_b200_decode_stack_workspace(int n_layers, int B, int d_model, int H, int S_max, int ffn);
-int it_b200_llama_decode_stack(int dtype, int n_layers, const itb_llama_layer *layers, const void *x_in,
-                               const void *position_id, int pos_flags, const void *rope_pos, int rope_pos_dtype,
-                               int B, int d_model, int H, int S_max, int ffn, void *workspace,
-                               int64_t workspace_bytes, void *stream);
-/* A chain of 1..8 skinny GEMM phases of the same persistent kernel (rows <= 16): phase p computes
- *      out[g] = xform_p(X_p)[rows, K_p] . W[g][K_p, n_per_group_p]   for its ngroups[p] weight matrices (W / out are the
- *      concatenation over phases), xform 0 none / 1 RMSNorm(norm_w) / 2 Silu(X) * X2, epi 0 store / 1 + residual.
- *      The wgmma decode GEMM on its own (logits head) and the unit under test of tests/test_gpu_decode_stack.py. ---- */
-/* stall diagnostics of the persistent kernel: returns a HOST pointer to 132 x 16 x 4 words that its wait sites report into
- * when a wait exceeds its budget (readable even after a trap killed the context); see tools/ds_debug.py */
-void *it_b200_decode_stack_debug(void);
-/* phase timeline of the persistent kernel: device buffer of >= 132 * n_phases * 2 uint64 (globaltimer at phase start /
- * this CTA's barrier arrival), NULL switches it off; see tools/ds_trace.py */
-void it_b200_decode_stack_trace(void *dev_buf);
-int it_b200_decode_gemm_chain(int dtype, int rows, int n_phases, const int *ngroups, const void *const *W,
-                              void *const *out, const int *n_per_group, const int *K, const int *xform,
-                              const int *epi, const void *const *X, const void *const *X2,
-                              const void *const *residual, const void *const *norm_w, void *workspace,
-                              int64_t workspace_bytes, void *stream);
-
 /* ======================================================================
  * (2) Graph / runtime handle API -- see infinitensor_b200/csrc/host/capi.cc.
  * Mirrors reference GraphHandlerObj (include/core/graph_handler.h:15-159),

@@ -88,20 +88,8 @@ _SIGS = {
     "it_b200_attention_prefill": (c_int, [c_int, vp, vp, vp, vp, c_int, c_int, c_int, c_int, c_int, vp, c_int, vp, c_int64, c_int64,
                                           c_int64, c_int64, vp]),
     "it_b200_attention_prefill_strided": (c_int, [c_int, vp, vp, vp, vp] + [c_int] * 5 + [vp, vp, vp, vp, vp, c_int, vp, c_int64, c_int64, c_int64, c_int64, vp]),
-    "it_b200_decode_stack_workspace": (c_int64, [c_int] * 6),
-    "it_b200_decode_stack_debug": (vp, []),
-    "it_b200_decode_stack_trace": (None, [vp]),
-    "it_b200_llama_decode_stack": (c_int, [c_int, c_int, vp, vp, vp, c_int, vp, c_int, c_int, c_int, c_int, c_int, c_int, vp,
-                                           c_int64, vp]),
-    "it_b200_decode_gemm_chain": (c_int, [c_int, c_int, c_int, i32p, POINTER(vp), POINTER(vp), i32p, i32p, i32p, i32p,
-                                          POINTER(vp), POINTER(vp), POINTER(vp), POINTER(vp), vp, c_int64, vp]),
 }
 
-
-class LlamaLayer(ctypes.Structure):
-    """itb_llama_layer (include/it_b200.h)"""
-    _fields_ = [(n, vp) for n in ("ln1_w", "wq", "wk", "wv", "wo", "ln2_w", "wg", "wu", "wd", "k_cache", "v_cache", "q", "k", "v",
-                                  "attn_out", "x_mid", "gate", "up", "x_out")]
 
 for _name, (_res, _args) in _SIGS.items():
     _f = getattr(lib, _name)

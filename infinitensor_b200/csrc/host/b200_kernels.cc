@@ -567,91 +567,6 @@ void runPrefillAttention(const OpVec &ops, const RuntimeObj *) {
                                  ms[0], ms[1], ms[2], ms[3], S()), mm2);
 }
 
-// DecoderStack: st.sub = per layer { RMSNorm | MatMulGroup{3} | AttentionRope | MatMulAdd | RMSNorm | MatMulGroup{2} | SiluMul |
-// MatMulAdd } with Alias steps in between (schedule.cc: matchDecoderLayer)
-bool runDecoderStack(const ExecStep &st, const RuntimeObj *ctx) {
-    vector<const ExecStep *> cs;
-    for (auto &sb : st.sub) {
-        if (sb.kind == ExecStep::Alias) {
-            // the kernel writes each tensor once: an alias must really share its input's storage (not the naive allocator)
-            if (sb.ops[0]->getInputs(0)->rawPtrOrNull() != sb.ops[0]->getOutput()->rawPtrOrNull()) return false;
-            continue;
-        }
-        cs.push_back(&sb);
-    }
-    if (cs.empty() || cs.size() % 8) return false;
-    const int L = (int)cs.size() / 8;
-    vector<itb_llama_layer> layers((size_t)L);
-    Tensor x0, pos, rpos;
-    Operator att0;
-    int B = 0, d = 0, H = 0, Smax = 0, f = 0;
-    for (int li = 0; li < L; ++li) {
-        const ExecStep *const *c = &cs[(size_t)li * 8];
-        auto n1 = c[0]->ops[0];
-        auto ropeQ = c[2]->ops[0], ropeK = c[2]->ops[1], att = c[2]->ops[2];
-        auto mo = c[3]->ops[0], add1 = c[3]->ops[1];
-        auto n2 = c[4]->ops[0];
-        auto silu = c[6]->ops[0], mul = c[6]->ops[1];
-        auto md = c[7]->ops[0], add2 = c[7]->ops[1];
-        Tensor qpre = ropeQ->getInputs(1), kpre = ropeK->getInputs(1);
-        Tensor vin = att->getInputs(4);
-        while (vin->getSource() && vin->getSource()->getOutput()->rawPtrOrNull() == vin->getSource()->getInputs(0)->rawPtrOrNull() &&
-               vin->getSource()->getOpType() != OpType::MatMul)
-            vin = vin->getSource()->getInputs(0);
-        Operator mq, mk, mv;
-        for (auto &mm : c[1]->ops) {
-            if (mm->getOutput() == qpre) mq = mm;
-            if (mm->getOutput() == kpre) mk = mm;
-            if (mm->getOutput() == vin) mv = mm;
-        }
-        if (!mq || !mk || !mv) return false;
-        Tensor gate = silu->getInputs(0);
-        Operator mg, mu;
-        for (auto &mm : c[5]->ops) (mm->getOutput() == gate ? mg : mu) = mm;
-        if (!mg || !mu) return false;
-        itb_llama_layer &Ly = layers[(size_t)li];
-        Ly.ln1_w = P(n1->getInputs(1));
-        Ly.wq = P(mq->getInputs(1));
-        Ly.wk = P(mk->getInputs(1));
-        Ly.wv = P(mv->getInputs(1));
-        Ly.wo = P(mo->getInputs(1));
-        Ly.ln2_w = P(n2->getInputs(1));
-        Ly.wg = P(mg->getInputs(1));
-        Ly.wu = P(mu->getInputs(1));
-        Ly.wd = P(md->getInputs(1));
-        Ly.k_cache = P(att->getInputs(0));
-        Ly.v_cache = P(att->getInputs(1));
-        Ly.q = P(qpre);
-        Ly.k = P(kpre);
-        Ly.v = P(vin);
-        Ly.attn_out = P(att->getOutput());
-        Ly.x_mid = P(add1->getOutput());
-        Ly.gate = P(mg->getOutput());
-        Ly.up = P(mu->getOutput());
-        Ly.x_out = P(add2->getOutput());
-        (void)mul;
-        if (li == 0) {
-            x0 = n1->getInputs(0);
-            pos = att->getInputs(5);
-            rpos = ropeQ->getInputs(0);
-            att0 = att;
-            const auto &cd = att->getInputs(0)->getDims();
-            B = cd[0];
-            H = cd[1];
-            Smax = cd[2];
-            d = x0->getDims().back();
-            f = as<MatmulObj>(mg)->getN();
-        }
-    }
-    auto rt = RT(ctx);
-    int64_t wsb = it_b200_decode_stack_workspace(L, B, d, H, Smax, f);
-    void *ws = rt->getWorkspace((size_t)wsb);
-    int rc = it_b200_llama_decode_stack(DTI(x0), L, layers.data(), P(x0), P(pos), attnPosFlags(att0, rpos), P(rpos), DTI(rpos), B, d, H, Smax, f,
-                                        ws, (int64_t)rt->getWorkspaceSize(), S());
-    CK(rc, att0);
-    return true;
-}
-
 // Conv -> BatchNorm -> [Add(residual)] -> [Relu]: ops = {conv, bn, [add], [relu]}; a lone Conv when ops.size() == 1.
 // layout (ExecStep::layout): bit 0 = x is NHWC -> implicit-GEMM kernel; bit 1 = y (and the residual) are NHWC
 bool runConvBnAct(const OpVec &ops, const RuntimeObj *ctx, int layout) {

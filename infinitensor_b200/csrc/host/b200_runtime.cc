@@ -199,9 +199,7 @@ void CudaRuntimeObj::runWithoutSyncImpl(const Graph &graph, bool validate) const
             Range(bool enable, const ExecStep &s) : on(enable) {
                 if (!on) return;
                 string name;
-                if (s.kind == ExecStep::DecoderStack) name = "DecoderStack";
-                else
-                    for (auto &m : s.ops) name += (name.empty() ? "" : "+") + string(m->getOpType().toString());
+                for (auto &m : s.ops) name += (name.empty() ? "" : "+") + string(m->getOpType().toString());
                 nvtxRangePushA(name.c_str());
             }
             ~Range() {
@@ -261,10 +259,6 @@ void CudaRuntimeObj::execStep(const ExecStep &st, Kernel *kernel, const PerfReco
             for (auto &m : st.ops) reg.getKernel(KernelAttrs{Device::CUDA, m->getOpType().underlying()})->compute(m, this);
         break;
     case ExecStep::PrefillAttention: b200::runPrefillAttention(st.ops, this); break;
-    case ExecStep::DecoderStack:
-        if (!b200::runDecoderStack(st, this))
-            for (auto &sb : st.sub) execStep(sb, nullptr, nullptr);
-        break;
     }
 }
 

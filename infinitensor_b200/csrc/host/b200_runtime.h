@@ -168,8 +168,6 @@ void runPoolNhwc(const Operator &op, const RuntimeObj *ctx);
 void runAttentionRope(const Operator &ropeQ, const Operator &ropeK, const Operator &att, const RuntimeObj *ctx);
 // {Transpose(k), MatMul, [Div | Mul], [Add], Softmax, MatMul} as one fused wgmma attention kernel
 void runPrefillAttention(const OpVec &ops, const RuntimeObj *ctx);
-// L decoder layers through the persistent kernel; false = not taken (nothing launched): run `st.sub` step by step
-bool runDecoderStack(const ExecStep &st, const RuntimeObj *ctx);
 }  // namespace b200
 
 // Convenience base for kernels without tunable configs (reference cuda_kernel_wihtout_config.h:7-22)

@@ -380,16 +380,10 @@ int itb_graph_step(itb_graph *g, int index, char *buf, int buf_len) {
     ITB_TRY({
         const auto &sc = g->g->getSchedule();
         IT_ASSERT(index >= 0 && index < (int)sc.size(), "bad step index");
-        static const char *kinds[] = {"Single", "Alias", "MatMulGroup", "MatMulAdd", "SiluMul", "AttentionRope", "AllReduceAddNorm", "ConvBnAct", "PrefillAttention", "DecoderStack"};
+        static const char *kinds[] = {"Single", "Alias", "MatMulGroup", "MatMulAdd", "SiluMul", "AttentionRope", "AllReduceAddNorm", "ConvBnAct", "PrefillAttention"};
         std::string s = kinds[(int)sc[index].kind];
         s += ":";
-        if (sc[index].kind == ExecStep::DecoderStack) {
-            // "<layers>xLayer(<launches replaced>)": the member operators would not fit a line
-            size_t compute = 0;
-            for (auto &sb : sc[index].sub) compute += sb.kind != ExecStep::Alias;
-            s += std::to_string(compute / 8) + "xLayer(" + std::to_string(compute) + " steps, " + std::to_string(sc[index].ops.size()) + " ops)";
-        } else
-            for (size_t i = 0; i < sc[index].ops.size(); ++i) s += (i ? "+" : "") + std::string(sc[index].ops[i]->getOpType().toString());
+        for (size_t i = 0; i < sc[index].ops.size(); ++i) s += (i ? "+" : "") + std::string(sc[index].ops[i]->getOpType().toString());
         // NHWC domain: "@nhwc" = operands and result channel-innermost, "@>nhwc" = enters the domain, "@nhwc>" = leaves it
         static const char *lay[] = {"", "@nhwc>", "@>nhwc", "@nhwc"};
         s += lay[sc[index].layout & 3];

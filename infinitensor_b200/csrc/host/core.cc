@@ -522,14 +522,10 @@ void GraphObj::dataMalloc(bool useNaiveAllocator, size_t memPoolSize) {
         }
     };
     if (!useNaiveAllocator) {
-        auto aliasOf = [&](const ExecStep &st) {
-            if (st.kind != ExecStep::Alias) return;
+        for (auto &st : sched) {
+            if (st.kind != ExecStep::Alias) continue;
             auto in = st.ops[0]->getInputs(0), out = st.ops[0]->getOutput();
             if (!in->isWeight() && !out->isWeight()) parent[out.get()] = in.get();
-        };
-        for (auto &st : sched) {
-            aliasOf(st);
-            for (auto &sb : st.sub) aliasOf(sb);  // aliases inside a DecoderStack step
         }
     }
     std::unordered_map<TensorObj *, int> refs;

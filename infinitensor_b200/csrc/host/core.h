@@ -369,14 +369,10 @@ struct ExecStep {
         AllReduceAddNorm, // AllReduceSum -> Add(residual) [-> RMSNorm]: one NVLink peer-memory kernel (else 3 ops)
         ConvBnAct,        // Conv -> BatchNorm -> [Add(residual)] -> [Relu]: the tail runs in the tensor-core GEMM epilogue
                           // (bit-identical to the separate kernels); shapes the GEMM does not take run one by one
-        PrefillAttention, // Transpose(k) -> MatMul(q, .) -> [Div | Mul scalar] -> [Add mask] -> Softmax(-1) -> MatMul(., v): one wgmma
+        PrefillAttention  // Transpose(k) -> MatMul(q, .) -> [Div | Mul scalar] -> [Add mask] -> Softmax(-1) -> MatMul(., v): one wgmma
                           // kernel per (batch, head, 128-query tile) (kernels/attention_prefill.cu); ops in that order
-        DecoderStack      // L consecutive Llama decoder layers (decode, <= 16 rows): ONE launch of the persistent kernel
-                          // (kernels/decode_stack.cu).  `sub` keeps the steps it replaces (8 launches + aliases per layer, in
-                          // order): executed one by one when the kernel does not take the shapes / storage
     } kind = Single;
     OpVec ops;
-    vector<ExecStep> sub;
     // NHWC domain (schedule.cc assignLayouts): bit 0 = the step's 4-D activation operands are stored [N, H, W, C], bit 1 = its
     // result is.  The tensors keep their logical NCHW dims; only Conv / Pool / same-shape Add / Relu steps carry these bits, and
     // graph inputs, outputs and every tensor some other operator reads stay NCHW.

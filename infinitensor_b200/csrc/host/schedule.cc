@@ -18,15 +18,12 @@ static bool fusionEnabled() {
 // (bit 9 = NHWC domain for Conv / Pool / Add / Relu chains, on by default)
 // (bit 10 = MatMul + bias -> [Gelu] -> [Add] in the wgmma epilogue, on by default)
 // (bit 11 = the head split / merge around a prefill-attention chain folded into the attention step, on by default)
-// ITB_FUSION_MASK (debug / A-B): bit 0 alias, 1 MatMul groups, 2 MatMul+Add, 3 Silu*Mul, 4 AllReduce+Add+Norm, 5 RoPE->Attention, 6 Conv+BatchNorm[+Add][+Relu], 7 decoder-layer stacks (persistent kernel); default all
+// ITB_FUSION_MASK (debug / A-B): bit 0 alias, 1 MatMul groups, 2 MatMul+Add, 3 Silu*Mul, 4 AllReduce+Add+Norm, 5 RoPE->Attention, 6 Conv+BatchNorm[+Add][+Relu], 7 unused; default all
 static int fusionMask() {
     const char *e = std::getenv("ITB_FUSION_MASK");
     if (e && e[0]) return std::atoi(e);
     // (bit 8 = prefill attention chains, on by default)
-    // bit 7 (decoder-layer stacks on the persistent kernel) is opt-in: it is not shown to beat the eight tuned launches it replaces
-    // -- ITB_DECODE_STACK=1 switches it on
-    const char *ds = std::getenv("ITB_DECODE_STACK");
-    return ((ds && ds[0] == '1') ? 255 : 127) | 256 | 512 | 1024 | 2048;
+    return 127 | 256 | 512 | 1024 | 2048;
 }
 
 static bool isKvCacheOperand(const Tensor &t) {
@@ -76,165 +73,6 @@ static bool groupableMatmul(const Operator &op) {
     if (B->getRank() != 2 || !B->isWeight()) return false;
     if (rowsOf(A) > 64) return false;  // decode regime: the grouped kernel is the skinny GEMM
     return true;
-}
-
-// ---------------------------------------------------------------------------------------------------------------------
-// Decoder-layer stacks.  After the per-operator fusions a Llama decode layer is this step sequence (Alias steps in between):
-//   Single RMSNorm | MatMulGroup{q,k,v} | AttentionRope{RoPE q, RoPE k, AttentionKVCache} | MatMulAdd{o, Add} |
-//   Single RMSNorm | MatMulGroup{gate, up} | SiluMul{Silu, Mul} | MatMulAdd{down, Add}
-// Consecutive layers with this exact data flow (<= 16 rows, q-len 1, 128-wide heads, f16 / bf16, constant weights, caches and
-// positions that are graph inputs of one shared position tensor) collapse into ONE DecoderStack step = one launch of the
-// persistent kernel; the replaced steps stay in `sub` for the fallback.  The kernel still writes q, k, v (pre-RoPE), the
-// attention output, both residual sums, gate and up; the RMSNorm / RoPE / Silu / Mul outputs are never materialised, so they
-// must have no other reader.
-static Tensor aliasRoot(Tensor t) {
-    while (true) {
-        auto src = t->getSource();
-        if (!src || !aliasable(src)) return t;
-        t = src->getInputs(0);
-    }
-}
-static bool soleUse(const Tensor &t, size_t n) { return !t->isOutput() && t->getTargets().size() == n; }
-
-struct LayerMatch {
-    size_t first, last;  // step indices [first, last]
-    Tensor xin, xout, pos, ropePos;
-    bool perRow;
-};
-
-static bool matchDecoderLayer(const vector<ExecStep> &s, size_t i, LayerMatch &m) {
-    auto nextCompute = [&](size_t j) {
-        while (j < s.size() && s[j].kind == ExecStep::Alias) ++j;
-        return j;
-    };
-    auto isHalf = [](const Tensor &t) { return t->getDType() == DataType::Float16 || t->getDType() == DataType::BFloat16; };
-    size_t j = nextCompute(i);
-    // (1) RMSNorm
-    if (j >= s.size() || s[j].kind != ExecStep::Single || s[j].ops[0]->getOpType() != OpType::RMSNorm) return false;
-    m.first = j;
-    auto n1 = s[j].ops[0];
-    Tensor x = n1->getInputs(0);
-    if (!isHalf(x) || !n1->getInputs(1)->isWeight() || x->getRank() < 2) return false;
-    const int d = x->getDims().back();
-    const int64_t rows = (int64_t)x->size() / d;
-    if (rows < 1 || rows > 16 || d % 8) return false;
-    if (!soleUse(n1->getOutput(), 3)) return false;
-    // (2) q / k / v
-    j = nextCompute(j + 1);
-    if (j >= s.size() || s[j].kind != ExecStep::MatMulGroup || s[j].ops.size() != 3) return false;
-    for (auto &mm : s[j].ops)
-        if (mm->getInputs(0) != n1->getOutput() || !mm->getInputs(1)->isWeight() || mm->getInputs(1)->getDType() != x->getDType()) return false;
-    const OpVec &qkv = s[j].ops;
-    // (3) RoPE + attention
-    j = nextCompute(j + 1);
-    if (j >= s.size() || s[j].kind != ExecStep::AttentionRope) return false;
-    auto ropeQ = s[j].ops[0], ropeK = s[j].ops[1], att = s[j].ops[2];
-    Tensor qpre = ropeQ->getInputs(1), kpre = ropeK->getInputs(1), vin = aliasRoot(att->getInputs(4));
-    Operator mq, mk, mv;
-    for (auto &mm : qkv) {
-        if (mm->getOutput() == qpre) mq = mm;
-        if (mm->getOutput() == kpre) mk = mm;
-        if (mm->getOutput() == vin) mv = mm;
-    }
-    if (!mq || !mk || !mv || mq == mk || mq == mv || mk == mv) return false;
-    if (!soleUse(qpre, 1) || !soleUse(kpre, 1) || !soleUse(vin, 1)) return false;
-    if (ropeQ->getInputs(0) != ropeK->getInputs(0)) return false;
-    auto kc = att->getInputs(0), vc = att->getInputs(1);
-    if (kc->getSource() || vc->getSource() || att->getInputs(5)->getSource() || ropeQ->getInputs(0)->getSource()) return false;
-    auto &cd = kc->getDims();
-    if (cd.size() != 4 || cd[3] != 128 || cd[0] != rows || kc->getDType() != x->getDType()) return false;
-    const int H = cd[1], dl = H * 128;
-    if (att->getInputs(2)->getDims()[1] != H) return false;  // grouped-query attention: the persistent kernel has one head count
-    for (auto &mm : qkv)
-        if (as<MatmulObj>(mm)->getN() != dl || as<MatmulObj>(mm)->getK() != d) return false;
-    if (!soleUse(att->getOutput(), 1)) return false;
-    m.pos = att->getInputs(5);
-    m.ropePos = ropeQ->getInputs(0);
-    m.perRow = as<AttentionKVCacheObj>(att)->getPerRowPositions();
-    // (4) o-proj + residual
-    j = nextCompute(j + 1);
-    if (j >= s.size() || s[j].kind != ExecStep::MatMulAdd) return false;
-    auto mo = as<MatmulObj>(s[j].ops[0]);
-    auto add1 = s[j].ops[1];
-    if (aliasRoot(mo->getInputs(0)) != att->getOutput() || !mo->getInputs(1)->isWeight() || mo->getTransA() || mo->getTransB() ||
-        mo->getBias() || mo->getK() != dl || mo->getN() != d || mo->getInputs(1)->getRank() != 2)
-        return false;
-    Tensor res1 = add1->getInputs(0) == mo->getOutput() ? add1->getInputs(1) : add1->getInputs(0);
-    if (res1 != x) return false;
-    Tensor x1 = add1->getOutput();
-    // (5) RMSNorm
-    j = nextCompute(j + 1);
-    if (j >= s.size() || s[j].kind != ExecStep::Single || s[j].ops[0]->getOpType() != OpType::RMSNorm) return false;
-    auto n2 = s[j].ops[0];
-    if (n2->getInputs(0) != x1 || !n2->getInputs(1)->isWeight() || !soleUse(n2->getOutput(), 2)) return false;
-    // (6) gate / up
-    j = nextCompute(j + 1);
-    if (j >= s.size() || s[j].kind != ExecStep::MatMulGroup || s[j].ops.size() != 2) return false;
-    const OpVec &gu = s[j].ops;
-    for (auto &mm : gu)
-        if (mm->getInputs(0) != n2->getOutput() || !mm->getInputs(1)->isWeight() || as<MatmulObj>(mm)->getK() != d) return false;
-    const int f = as<MatmulObj>(gu[0])->getN();
-    if (as<MatmulObj>(gu[1])->getN() != f || f % 8) return false;
-    // (7) Silu * Mul
-    j = nextCompute(j + 1);
-    if (j >= s.size() || s[j].kind != ExecStep::SiluMul) return false;
-    auto silu = s[j].ops[0], mul = s[j].ops[1];
-    Tensor gate = silu->getInputs(0);
-    Tensor up = mul->getInputs(0) == silu->getOutput() ? mul->getInputs(1) : mul->getInputs(0);
-    if (!((gate == gu[0]->getOutput() && up == gu[1]->getOutput()) || (gate == gu[1]->getOutput() && up == gu[0]->getOutput()))) return false;
-    if (!soleUse(gate, 1) || !soleUse(up, 1) || !soleUse(silu->getOutput(), 1) || !soleUse(mul->getOutput(), 1)) return false;
-    // (8) down + residual
-    j = nextCompute(j + 1);
-    if (j >= s.size() || s[j].kind != ExecStep::MatMulAdd) return false;
-    auto md = as<MatmulObj>(s[j].ops[0]);
-    auto add2 = s[j].ops[1];
-    if (md->getInputs(0) != mul->getOutput() || !md->getInputs(1)->isWeight() || md->getTransA() || md->getTransB() || md->getBias() ||
-        md->getK() != f || md->getN() != d || md->getInputs(1)->getRank() != 2)
-        return false;
-    Tensor res2 = add2->getInputs(0) == md->getOutput() ? add2->getInputs(1) : add2->getInputs(0);
-    if (res2 != x1) return false;
-    // every weight matrix is [K, N] (no transposes) and rank 2 -- the grouped matcher already guarantees it for q/k/v, gate/up
-    m.last = j;
-    m.xin = x;
-    m.xout = add2->getOutput();
-    return true;
-}
-
-static void fuseDecoderStacks(vector<ExecStep> &sched) {
-    vector<ExecStep> out;
-    size_t i = 0;
-    while (i < sched.size()) {
-        LayerMatch m;
-        if (sched[i].kind != ExecStep::Alias && matchDecoderLayer(sched, i, m) && m.first == i) {
-            ExecStep st;
-            st.kind = ExecStep::DecoderStack;
-            LayerMatch cur = m;
-            size_t end = m.last;
-            while (true) {
-                for (size_t k = i; k <= end; ++k) {
-                    st.sub.push_back(sched[k]);
-                    for (auto &o : sched[k].ops) st.ops.push_back(o);
-                }
-                i = end + 1;
-                // the next layer must start right here (only aliases in between) and continue the same residual stream
-                size_t j = i;
-                while (j < sched.size() && sched[j].kind == ExecStep::Alias) ++j;
-                LayerMatch nx;
-                if (j < sched.size() && matchDecoderLayer(sched, j, nx) && nx.first == j && nx.xin == cur.xout && nx.pos == m.pos &&
-                    nx.ropePos == m.ropePos && nx.perRow == m.perRow) {
-                    cur = nx;
-                    end = nx.last;
-                    continue;
-                }
-                break;
-            }
-            out.push_back(std::move(st));
-            continue;
-        }
-        out.push_back(sched[i]);
-        ++i;
-    }
-    sched.swap(out);
 }
 
 // Multi-token attention as the frontend lowers it (no fused op exists in the reference for q-len > 1):
@@ -745,7 +583,6 @@ const vector<ExecStep> &GraphObj::getSchedule() {
         }
         schedule.push_back(std::move(st));
     }
-    if (fuse && (mask & 128)) fuseDecoderStacks(schedule);
     if (fuse && (mask & 512)) LayoutPass().run(schedule);
     // every operator is executed by exactly one step (a producer parked behind a consumer that never runs would be a
     // silently skipped op)

@@ -15,7 +15,7 @@ Bounds (u = 2^-24).  The library is built without fast-math, so the fp32 emulati
 float64, out = rnd_T(rnd_T(sum p) + r): each rounding to T within ulp_T of its exact value (a whole ulp covers a rounding
 that crosses a binade), plus the fp32 chain of W - 1 additions, each within u of a partial sum no larger than sum |p|:
     |out - (sum p + r)| <= (W - 1) u sum|p| + ulp_T(sum p) [+ ulp_T(sum p + r)]
-out_norm is held to stack64.rmsnorm_operand's interval from the kernel's own `out` (rinv's fp32 window for a chain of
+out_norm is held to operand64.rmsnorm_operand's interval from the kernel's own `out` (rinv's fp32 window for a chain of
 `items + 10` roundings: the thread's items, then block_sum's two 5-level warp trees), and to a ratio bound `norm_bound`.
 
 Work partition.  The fused kernel runs threads = min(512, roundup32(nv)) per row (nv = H / V vectors of 16 bytes, V = 16 /
@@ -26,7 +26,7 @@ for bit (`partitions_coincide`).
 """
 import numpy as np
 
-from tests import ref64, stack64
+from tests import operand64, ref64
 from tests.gpt2_64 import rnd
 from tests.ref64 import BF16, F16, F32
 
@@ -100,10 +100,10 @@ def _block_sum(ss, threads):
     """block_sum over [rows, threads] per-thread sums: warp butterflies, then one over the warp sums (zero-padded to 32)"""
     m = ss.shape[0]
     nw = -(-threads // 32)
-    warps = stack64._xor_tree(ss.reshape(m, nw, 32), 5)
+    warps = operand64._xor_tree(ss.reshape(m, nw, 32), 5)
     red = np.zeros((m, 32), np.float32)
     red[:, :nw] = warps
-    return stack64._xor_tree(red, 5)
+    return operand64._xor_tree(red, 5)
 
 
 def emu_rinv(x, dt, eps=True):
@@ -200,20 +200,20 @@ def out_ref(P, R, dt):
 
 
 def norm_chain(dt, H):
-    return stack64.chain_length("block", H, items=ar_items(dt, H))
+    return operand64.chain_length("block", H, items=ar_items(dt, H))
 
 
 def norm_operand(out, w, dt):
-    """stack64's interval operand of rnd(rnd(out rinv) w) for the fused kernel's chain"""
-    return stack64.rmsnorm_operand(out, w, dt, norm_chain(dt, out.shape[1]))
+    """operand64's interval operand of rnd(rnd(out rinv) w) for the fused kernel's chain"""
+    return operand64.rmsnorm_operand(out, w, dt, norm_chain(dt, out.shape[1]))
 
 
 def norm_bound(out, w, dt):
     """ref = out rinv w in float64; bound: the two roundings (whole ulps) and rinv's fp32 window carried through w"""
     x, w = np.asarray(out, np.float64), np.asarray(w, np.float64)[None, :]
-    y = x * stack64.rinv64(x)
+    y = x * operand64.rinv64(x)
     ref = y * w
-    bound = ref64.ulp(ref, dt) + np.abs(w) * (ref64.ulp(y, dt) + stack64.rms_window(norm_chain(dt, x.shape[1])) * np.abs(y))
+    bound = ref64.ulp(ref, dt) + np.abs(w) * (ref64.ulp(y, dt) + operand64.rms_window(norm_chain(dt, x.shape[1])) * np.abs(y))
     return Ref(ref, bound, ref)
 
 
@@ -257,7 +257,7 @@ def inputs(dt, W, M, H, regime, seed, residual=True, norm=True):
         P[rng.integers(0, W), np.arange(M), col] = huge
     P = rnd(P, dt).astype(np.float32)
     R = None if R is None else rnd(R, dt).astype(np.float32)
-    w = stack64.norm_weight(H, dt, seed + 7).astype(np.float32) if norm else None
+    w = operand64.norm_weight(H, dt, seed + 7).astype(np.float32) if norm else None
     return P, R, w
 
 

@@ -12,7 +12,7 @@ slot (e & 1, p, row), nothing else written), the timeout flag must be 0, `out` a
 rank, guards after them untouched and the inputs unchanged.
 
 * out: bit for bit against ar64.emulate and within ar64.out_ref's float64 bound;
-* out_norm: inside stack64.rmsnorm_operand's interval from the kernel's own out, within ar64.norm_bound, and bit for bit equal
+* out_norm: inside operand64.rmsnorm_operand's interval from the kernel's own out, within ar64.norm_bound, and bit for bit equal
   to it_b200_rmsnorm / _constw of the same out where the two kernels' per-thread partitions coincide;
 * epochs: zero, per-row epochs of both parities in one launch, sequences of rounds with M and the order varying on the same
   workspaces, and a sequence through the wrap at INT_MAX (the epoch arithmetic is unsigned).

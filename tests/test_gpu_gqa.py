@@ -173,13 +173,6 @@ def test_gqa_llama3_width_graph_parity():
     run_gqa_llama_parity(cfg, pos=511, steps=1)
 
 
-def test_gqa_graph_with_decode_stack_requested(monkeypatch):
-    """ITB_DECODE_STACK=1 leaves a GQA layer to the per-operator steps, and the graph still matches"""
-    monkeypatch.setenv("ITB_DECODE_STACK", "1")
-    _, sched = run_gqa_llama_parity(_gqa_cfg(BF16, 2), pos=5, steps=2)
-    assert not any(s.startswith("DecoderStack") for s in sched)
-
-
 def _ngpu():
     import torch
     return torch.cuda.device_count() if torch.cuda.is_available() else 0

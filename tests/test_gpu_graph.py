@@ -36,30 +36,6 @@ def test_llama_decode_baseline_width():
     run_llama_parity(cfg=cfg, pos=511, steps=1)
 
 
-@pytest.mark.parametrize("dtype,cudagraph", [(BF16, True), (F16, False)])
-def test_llama_decode_stack_in_graph(dtype, cudagraph, monkeypatch):
-    """ITB_DECODE_STACK=1: the decoder layers run as ONE launch of the persistent kernel (DecoderStack step) inside the graph --
-    schedule, planner (aliases inside the step), CUDA-graph capture of the cached program, three steps against the oracle."""
-    monkeypatch.setenv("ITB_DECODE_STACK", "1")
-    from infinitensor_b200 import backend as B, graphs as G
-    from tests.smoke_impl import run_llama_parity
-    cfg = G.LlamaConfig(layers=3, d_model=512, heads=4, head_dim=128, ffn=1408, vocab=512, s_max=64, batch=16, dtype=dtype)
-    h = B.GraphHandler(B.CudaRuntime(0))
-    G.build_llama_decode(h, cfg)
-    assert any(s.startswith("DecoderStack:3xLayer") for s in h.schedule())
-    worst, launches = run_llama_parity(cfg=cfg, pos=9, steps=3, cudagraph=cudagraph)
-    assert launches > 0
-
-
-def test_llama_decode_stack_baseline_width(monkeypatch):
-    """The BASELINE per-layer shapes through the DecoderStack step, two layers, against the oracle."""
-    monkeypatch.setenv("ITB_DECODE_STACK", "1")
-    from infinitensor_b200 import graphs as G
-    from tests.smoke_impl import run_llama_parity
-    cfg = G.LlamaConfig(layers=2, d_model=4096, heads=32, head_dim=128, ffn=11008, vocab=32000, s_max=1024, batch=16, dtype=BF16)
-    run_llama_parity(cfg=cfg, pos=511, steps=1)
-
-
 @pytest.mark.parametrize("dtype", [BF16, F16])
 def test_llama_decode_fp8_weights(dtype):
     """SURVEY 8(f-4) through the graph: every projection (q/k/v grouped, o + residual, gate/up grouped, down + residual, logits)

@@ -47,8 +47,8 @@ def _cfg(kv_heads, **kw):
     return G.LlamaConfig(kv_heads=kv_heads, **base)
 
 
-def test_gqa_llama_schedule(B, monkeypatch):
-    """both RoPEs fold into one AttentionRope step per layer; ITB_DECODE_STACK=1 forms no DecoderStack"""
+def test_gqa_llama_schedule(B):
+    """both RoPEs fold into one AttentionRope step per layer"""
     from infinitensor_b200 import graphs as G
     rt = B.HostPlanRuntime()
     for kv in (2, 1):
@@ -62,26 +62,21 @@ def test_gqa_llama_schedule(B, monkeypatch):
         kinds = collections.Counter(s.split(":")[0] for s in sc)
         assert kinds["AttentionRope"] == 2 and kinds["MatMulGroup"] == 4
         h.data_malloc()
-    monkeypatch.setenv("ITB_DECODE_STACK", "1")
     h = B.GraphHandler(rt)
     G.build_llama_decode(h, _cfg(2))
-    assert not any(s.startswith("DecoderStack") for s in h.schedule())
     assert sum(s.startswith("AttentionRope") for s in h.schedule()) == 2
 
 
-def test_equal_heads_schedule_unchanged(B, monkeypatch):
+def test_equal_heads_schedule_unchanged(B):
     """kv_heads=None and kv_heads=heads build the very graph the equal-heads builder always built"""
     from infinitensor_b200 import graphs as G
     rt = B.HostPlanRuntime()
-    for env in (None, "1"):
-        if env:
-            monkeypatch.setenv("ITB_DECODE_STACK", env)
-        scheds = []
-        for kv in (None, 4):
-            h = B.GraphHandler(rt)
-            G.build_llama_decode(h, _cfg(kv))
-            scheds.append(h.schedule())
-        assert scheds[0] == scheds[1]
+    scheds = []
+    for kv in (None, 4):
+        h = B.GraphHandler(rt)
+        G.build_llama_decode(h, _cfg(kv))
+        scheds.append(h.schedule())
+    assert scheds[0] == scheds[1]
     assert G.LlamaConfig().algorithmic_bytes(511) == G.LlamaConfig(kv_heads=32).algorithmic_bytes(511)
     assert G.LlamaConfig().weight_elems() == G.LlamaConfig(kv_heads=32).weight_elems()
 

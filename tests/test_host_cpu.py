@@ -392,18 +392,6 @@ def test_fused_schedule_and_alias_plan(B, monkeypatch):
     from infinitensor_b200 import graphs as G
     rt = B.HostPlanRuntime()
     cfg = G.LlamaConfig(layers=2, d_model=512, heads=4, head_dim=128, ffn=1024, vocab=128, s_max=32, batch=16)
-    # ITB_DECODE_STACK=1: the two decoder layers collapse into ONE step of the persistent kernel (gather, final norm, logits remain)
-    monkeypatch.setenv("ITB_DECODE_STACK", "1")
-    h0 = B.GraphHandler(rt)
-    G.build_llama_decode(h0, cfg)
-    sc0 = [s for s in h0.schedule() if not s.startswith("Alias")]
-    assert sc0 == ["Single:Gather", "DecoderStack:2xLayer(16 steps, 48 ops)", "Single:RMSNorm", "Single:MatMul"], sc0
-    h0.data_malloc()
-    # a batch beyond the kernel's 16 rows, or a layer whose intermediate is a graph output, keeps the per-operator steps
-    hb = B.GraphHandler(rt)
-    G.build_llama_decode(hb, G.LlamaConfig(layers=1, d_model=512, heads=4, head_dim=128, ffn=1024, vocab=128, s_max=32, batch=17))
-    assert not any(s.startswith("DecoderStack") for s in hb.schedule())
-    monkeypatch.delenv("ITB_DECODE_STACK")  # default: the per-operator fusions
     h = B.GraphHandler(rt)
     G.build_llama_decode(h, cfg)
     sc = h.schedule()
@@ -420,7 +408,6 @@ def test_fused_schedule_and_alias_plan(B, monkeypatch):
     assert sc_tp.count("AllReduceAddNorm:AllReduceSum+Add+RMSNorm") == 4 and sc_tp.count("Single:RMSNorm") == 1
     h.data_malloc()
     fused_bytes = h.arena_bytes()[1]
-    assert h0.arena_bytes()[1] <= 1.5 * fused_bytes  # a stack keeps its layers' intermediates live together (~1.5 MB per 7B layer)
     monkeypatch.setenv("ITB_NO_FUSION", "1")
     h2 = B.GraphHandler(rt)
     G.build_llama_decode(h2, cfg)

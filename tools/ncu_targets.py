@@ -1,7 +1,6 @@
 #!/usr/bin/env python
-"""Small single-process workloads for ncu captures (profiles/r02_*):  python tools/ncu_targets.py llama|stack|prefill|resnet
+"""Small single-process workloads for ncu captures (profiles/r02_*):  python tools/ncu_targets.py llama|prefill|resnet
    llama   : one eager pass of a 1-layer BASELINE-width Llama decode graph (q/k/v group, attention, o, gate/up group, down, logits GEMMs)
-   stack   : the same two layers deep through the persistent decode kernel (ITB_DECODE_STACK=1)
    prefill : GPT-2's attention block shape through attention_prefill_kernel
    resnet  : ResNet-50 B = 64 fp16, two eager passes"""
 import ctypes
@@ -13,8 +12,6 @@ import numpy as np
 import torch
 
 what = sys.argv[1] if len(sys.argv) > 1 else "llama"
-if what == "stack":
-    os.environ["ITB_DECODE_STACK"] = "1"
 from infinitensor_b200 import backend as B, graphs as G, _lib as L
 
 
@@ -39,8 +36,6 @@ def llama(layers):
 
 if what == "llama":
     llama(1)
-elif what == "stack":
-    llama(2)
 elif what == "prefill":
     q, k, v = (torch.randn(1, 12, 128, 64, device="cuda").half() for _ in range(3))
     out = torch.zeros_like(q)
