@@ -318,6 +318,20 @@ int it_b200_attention_kvcache_gqa(int dtype, void *k_cache, void *v_cache, const
                                   int B, int Hq, int Hkv, int S_max, int D, void *workspace, int64_t workspace_bytes,
                                   void *stream);
 
+/* ---- AttentionKVCache over a prompt chunk of S >= 1 new tokens (attention_prefill.cu): exactly S single-token AttentionKVCache
+ *      calls in order, token i of batch row b at position p_b + i.  Caches [B,Hkv,S_max,D]; q / out [B,Hq,S,D]; k / v [B,Hkv,S,D];
+ *      Hq = G * Hkv.  Token i's k / v are copied into cache row p_b + i; query i of head h attends over rows 0 .. p_b + i of KV
+ *      head h / G with scale 1/sqrt(D) (causal attention with an offset: also chunked prefill, p_b > 0).  p_b is element 0 of
+ *      position_id, or with ITB_POS_PER_ROW element b * stride (stride = pos_flags >> ITB_POS_ROW_STRIDE_SHIFT, 0 meaning 1: a
+ *      [B, S] position tensor has stride S); positions inside a row are taken to be consecutive, only the start is read.
+ *      p_b is clamped to [0, S_max - S]; S > S_max is refused.  f16 / bf16 only (fp32 is refused), D = 64 or 128.  Two launches
+ *      (append, then attention, PDL-chained); nothing is read before griddepcontrol.wait, so ITB_POS_IN_STEP changes nothing.
+ *      No workspace. ---- */
+#define ITB_POS_ROW_STRIDE_SHIFT 16
+int it_b200_attention_kvcache_prompt(int dtype, void *k_cache, void *v_cache, const void *q, const void *k, const void *v,
+                                     const void *position_id, int pos_flags, void *out, int B, int Hq, int Hkv, int S, int S_max,
+                                     int D, void *stream);
+
 /* ---- Fused prefill attention (q-len > 1) on wgmma (SURVEY 8(f-3); attention_prefill.cu):
  *      out[b,h] = softmax((q . k^T) (/ or *) scale + mask) . v, q / k / v / out [B, H, S, D] f16 / bf16, D = 64 or 128.
  *      Replaces the chain the frontend lowers multi-token attention to -- Transpose(k) -> MatMul (matmul.cc:66-211) ->

@@ -507,6 +507,13 @@ static int attnPosFlags(const Operator &att, const Tensor &ropePos) {
     if (as<AttentionKVCacheObj>(att)->getPerRowPositions()) {
         IT_ASSERT((int64_t)pos->size() >= att->getInputs(0)->getDims()[0], "AttentionKVCache: per-row positions need one entry per batch row");
         flags |= ITB_POS_PER_ROW;
+        // a prompt chunk (S > 1) reads row b's first position at flat index b * (elements per row): [B, S] positions, as RoPE
+        // takes them, have stride S, [B, 1] stride 1
+        if (att->getInputs(2)->getDims()[2] > 1) {
+            const int64_t stride = (int64_t)pos->size() / att->getInputs(0)->getDims()[0];
+            IT_ASSERT(stride < (1 << (31 - ITB_POS_ROW_STRIDE_SHIFT)), "AttentionKVCache: per-row position stride beyond the flag field");
+            flags |= (int)stride << ITB_POS_ROW_STRIDE_SHIFT;
+        }
     }
     bool inStep = pos->getSource() != nullptr || att->getInputs(0)->getSource() != nullptr || att->getInputs(1)->getSource() != nullptr;
     if (ropePos && ropePos->getSource() != nullptr) inStep = true;
@@ -765,6 +772,16 @@ class AttentionKVCacheB200 : public CudaKernelWithoutConfig {
              v = op->getInputs(4), pos = op->getInputs(5);
         const auto &d = kc->getDims();
         const int hq = q->getDims()[1];  // = G x the caches' d[1] KV heads
+        if (const int seq = q->getDims()[2]; seq > 1) {  // a prompt chunk: append + causal attention over the cache
+            CK(it_b200_attention_kvcache_prompt(DTI(q), P(kc), P(vc), P(q), P(k), P(v), P(pos),
+#ifdef ITB_SEAM_A
+                                                DTI(pos),
+#else
+                                                b200::attnPosFlags(op, nullptr),
+#endif
+                                                P(op->getOutput()), d[0], hq, d[1], seq, d[2], d[3], S()), op);
+            return;
+        }
         int64_t wsb = it_b200_attention_kvcache_workspace(d[0], hq, d[2], d[3]);
         void *ws = wsb ? RT(ctx)->getWorkspace((size_t)wsb) : nullptr;
         CK(it_b200_attention_kvcache_gqa(DTI(q), P(kc), P(vc), P(q), P(k), P(v), P(pos),

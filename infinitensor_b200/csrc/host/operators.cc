@@ -101,6 +101,14 @@ std::optional<vector<Shape>> AttentionKVCacheObj::inferShape(const TensorVec &in
     IT_ASSERT(k[2] == q[2], "AttentionKVCache: q and k / v lengths differ");
     IT_ASSERT(k[1] == c[1], "AttentionKVCache: k / v head count differs from the caches'");
     IT_ASSERT(c[1] > 0 && q[1] % c[1] == 0, "AttentionKVCache: query heads are not a multiple of the caches' KV heads");
+    if (q[2] > 1) {  // a prompt chunk of S tokens at positions p_b .. p_b + S - 1
+        IT_ASSERT(q[2] <= c[2], "AttentionKVCache: " + std::to_string(q[2]) + " new tokens do not fit a cache of " +
+                                    std::to_string(c[2]) + " rows");
+        IT_ASSERT(ins[2]->getDType() != DataType::Float32, "AttentionKVCache: fp32 takes one token per step (S = 1)");
+        const int64_t np = (int64_t)ins[5]->size();
+        IT_ASSERT(np == (int64_t)q[0] || np == (int64_t)q[0] * q[2],
+                  "AttentionKVCache: a prompt chunk takes one position per batch row or one per token");
+    }
     return {{ins[2]->getDims()}};
 }
 

@@ -395,6 +395,258 @@ static int launch_ap(const void *q, const void *k, const void *v, ApArgs a, cuda
     return 0;
 }
 
+// ------------------------------------------------------------------------------------------------------------------
+// AttentionKVCache over a prompt chunk of S > 1 tokens (it_b200_attention_kvcache_prompt): S single-token AttentionKVCache
+// steps in order, token i of batch row b at position p_b + i.  Two launches, the second PDL-chained behind the first:
+//   kvcache_append_kernel      copies k / v [B, Hkv, S, D] into cache rows [p_b, p_b + S), bit for bit;
+//   attention_kvcache_prompt_kernel  one CTA (one warpgroup) per (batch row, query head, 64-query tile): causal attention
+//                                    of the tile's queries over cache rows 0 .. p_b + i of KV head h / G.
+// The attention kernel reads the cache only after griddepcontrol.wait, so every row it reads, the appended ones included,
+// is complete; no CTA writes what another reads.  Per 64-key tile:
+//   S = Q K^T   wgmma m64n64k16 (D / 16 steps, fp32 accumulators), Q and K by TMA (128B swizzle), scaled by fp32 1/sqrt(D)
+//               like the decode kernels; key j of query i is kept when j <= p_b + i (only the diagonal tiles test it; key
+//               tiles wholly past the tile's last query are never loaded);
+//   softmax     online over the key tiles in fp32 (row max and sum across the 4 lanes of a fragment row);
+//   O += P V    P enters the tensor core as hi = P rounded to T and lo = P - hi rounded to T, two wgmma chains into the
+//               same fp32 accumulator (16 / 22 significant bits per weight for bf16 / f16, as attn_gqa_kernel keeps them);
+//               V is the MN-major B operand straight from its [keys, D] tile.
+// The output leaves the registers once, O / l rounded to T.  Query heads of one KV head run in separate CTAs (simpler
+// than packing G heads x tokens into the M rows as attn_gqa_kernel does): each K / V tile is fetched once per query head,
+// the repeats mostly from L2.  K / V tiles are double-buffered.
+// ------------------------------------------------------------------------------------------------------------------
+constexpr int PK_BQ = 64, PK_BK = 64, PK_THREADS = 128;
+
+struct PkArgs {
+    const void *pos;
+    int pos_flags;  // ITB_I32 / ITB_U32 / ITB_I64 | ITB_POS_PER_ROW, row stride in bits ITB_POS_ROW_STRIDE_SHIFT..
+    void *out;      // [B, Hq, S, D]
+    int Hq, Hkv, G, S, Smax;
+};
+
+// p_b: element 0 of the positions, or (ITB_POS_PER_ROW) row b's first element at flat index b * stride; clamped to
+// [0, Smax - S] so that rows [p_b, p_b + S) lie in the cache
+__device__ __forceinline__ int prompt_start(const void *pos, int flags, int b, int S, int Smax) {
+    const int stride = max(flags >> ITB_POS_ROW_STRIDE_SHIFT, 1);
+    const int64_t i = (flags & ITB_POS_PER_ROW) ? (int64_t)b * stride : 0;
+    const int64_t p = (flags & 0xff) == ITB_I64 ? ((const int64_t *)pos)[i] : (int64_t)((const int32_t *)pos)[i];
+    return (int)min(max(p, (int64_t)0), (int64_t)(Smax - S));
+}
+
+// grid (ceil(S D / 8 / 256), B Hkv): one 16-byte chunk of k and of v per thread
+template <typename T>
+__global__ void __launch_bounds__(256) kvcache_append_kernel(T *__restrict__ kc, T *__restrict__ vc, const T *__restrict__ k,
+                                                             const T *__restrict__ v, const void *pos, int pos_flags, int Hkv,
+                                                             int S, int Smax, int D) {
+    pdl_trigger();
+    pdl_wait();
+    const int bh = blockIdx.y, b = bh / Hkv;
+    const int64_t n = (int64_t)S * D / 8, c = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (c >= n) return;
+    const int p = prompt_start(pos, pos_flags, b, S, Smax);
+    const int64_t src = (int64_t)bh * S * D / 8 + c, dst = ((int64_t)bh * Smax + p) * D / 8 + c;
+    reinterpret_cast<uint4 *>(kc)[dst] = reinterpret_cast<const uint4 *>(k)[src];
+    reinterpret_cast<uint4 *>(vc)[dst] = reinterpret_cast<const uint4 *>(v)[src];
+}
+
+template <typename T, int D>
+__global__ void __launch_bounds__(PK_THREADS, 1) attention_kvcache_prompt_kernel(const __grid_constant__ CUtensorMap mapQ,
+                                                                                 const __grid_constant__ CUtensorMap mapK,
+                                                                                 const __grid_constant__ CUtensorMap mapV,
+                                                                                 const PkArgs a) {
+    constexpr int DG = D / 64;                  // 64-column groups of the head dim
+    constexpr int TILE_BYTES = PK_BQ * D * 2;   // a Q, K or V tile: DG boxes of [64 rows x 64 columns], 128B swizzle
+    constexpr int P_BYTES = PK_BQ * PK_BK * 2;  // P hi or lo: [64 queries x 64 keys], K-major, 128B swizzle
+    constexpr float kScale = D == 128 ? 0.08838834764831845f : 0.125f;  // fp32 1/sqrt(D), as the decode kernels
+    extern __shared__ uint8_t pk_smem_raw[];
+    uint8_t *smem = pk_smem_raw + ((1024u - (smem_u32(pk_smem_raw) & 1023u)) & 1023u);
+    uint8_t *q_sm = smem, *kv_sm = q_sm + TILE_BYTES;  // kv_sm: stage s = { K tile, V tile } at 2 s TILE_BYTES
+    uint8_t *ph_sm = kv_sm + 4 * TILE_BYTES, *pl_sm = ph_sm + P_BYTES;
+    __shared__ __align__(8) uint64_t bar_q, bar_kv[2];
+
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int qt = gridDim.x - 1 - blockIdx.x;  // the longest (last) query tiles start first
+    const int bh = blockIdx.y, b = bh / a.Hq, h = bh % a.Hq;
+    const int kvh = b * a.Hkv + h / a.G;
+    const int i0 = qt * PK_BQ;
+    pdl_trigger();
+    if (threadIdx.x == 0) {
+        mbar_init(&bar_q, 1);
+        mbar_init(&bar_kv[0], 1);
+        mbar_init(&bar_kv[1], 1);
+        fence_mbar_init();
+        tma_prefetch_desc(&mapQ);
+        tma_prefetch_desc(&mapK);
+        tma_prefetch_desc(&mapV);
+    }
+    __syncthreads();
+    pdl_wait();  // q / k / v and every cache row >= p_b are written in this step (the append launch)
+
+    const int p = prompt_start(a.pos, a.pos_flags, b, a.S, a.Smax);
+    const int last = p + min(i0 + PK_BQ - 1, a.S - 1);  // the tile's last query attends over rows 0 .. last
+    const int nkt = last / PK_BK + 1;
+    const uint64_t pol = l2_policy_evict_last();
+    auto load_kv = [&](int t) {
+        uint8_t *ks = kv_sm + (t & 1) * 2 * TILE_BYTES, *vs = ks + TILE_BYTES;
+        mbar_expect_tx(&bar_kv[t & 1], 2 * TILE_BYTES);
+#pragma unroll
+        for (int g = 0; g < DG; ++g) {
+            tma_load_3d(ks + g * (PK_BK * 128), &mapK, &bar_kv[t & 1], g * 64, t * PK_BK, kvh, pol);
+            tma_load_3d(vs + g * (PK_BK * 128), &mapV, &bar_kv[t & 1], g * 64, t * PK_BK, kvh, pol);
+        }
+    };
+    if (threadIdx.x == 0) {
+        mbar_expect_tx(&bar_q, TILE_BYTES);
+#pragma unroll
+        for (int g = 0; g < DG; ++g) tma_load_3d(q_sm + g * (PK_BQ * 128), &mapQ, &bar_q, g * 64, i0, bh, pol);
+        load_kv(0);
+    }
+
+    // accumulator fragment: d[4 j + 2 r + e] is row 16 warp + lane / 4 + 8 r, column 8 j + 2 (lane % 4) + e
+    const int fr = 16 * warp + (lane >> 2), fc = 2 * (lane & 3);
+    int lim[2];  // per fragment row: the last key it attends to (rows past S behave like row S - 1; they are not stored)
+#pragma unroll
+    for (int r = 0; r < 2; ++r) lim[r] = p + min(i0 + fr + 8 * r, a.S - 1);
+    float o[DG][32];
+#pragma unroll
+    for (int g = 0; g < DG; ++g)
+#pragma unroll
+        for (int j = 0; j < 32; ++j) o[g][j] = 0.f;
+    float m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};
+    mbar_wait(&bar_q, 0);
+
+    for (int t = 0; t < nkt; ++t) {
+        if (threadIdx.x == 0 && t + 1 < nkt) load_kv(t + 1);  // (stage (t + 1) & 1 was released by the barrier closing t - 1)
+        uint8_t *ks = kv_sm + (t & 1) * 2 * TILE_BYTES, *vs = ks + TILE_BYTES;
+        mbar_wait(&bar_kv[t & 1], (t >> 1) & 1);
+        const int j0 = t * PK_BK;
+        // V rows past p_b + S - 1 (the last tile only) are cache contents this step does not own, possibly non-finite: they
+        // meet P = 0 in the product, so they are zeroed here
+        if (j0 + PK_BK > p + a.S) {
+            const int r0 = p + a.S - j0;
+            for (int c = threadIdx.x; c < (PK_BK - r0) * DG * 8; c += PK_THREADS) {
+                const int r = r0 + c / (DG * 8), g = (c / 8) % DG, ch = c % 8;
+                *reinterpret_cast<uint4 *>(vs + g * (PK_BK * 128) + r * 128 + ch * 16) = make_uint4(0, 0, 0, 0);
+            }
+            fence_proxy_async();
+        }
+
+        float s[32];
+#pragma unroll
+        for (int j = 0; j < 32; ++j) s[j] = 0.f;
+        wg_fence();
+#pragma unroll
+        for (int kk = 0; kk < D / 16; ++kk) {
+            const uint32_t off = (kk >> 2) * (PK_BK * 128) + (kk & 3) * 32;
+            Wgmma<T, 64>::template mma<0, 0>(s, gmma_desc_sw128(smem_u32(q_sm) + off, 0, 1024),
+                                             gmma_desc_sw128(smem_u32(ks) + off, 0, 1024), 1u);
+        }
+        wg_commit();
+        wg_wait<0>();
+
+        const bool diag = j0 + PK_BK - 1 > p + i0;  // some key of the tile lies past the first query's limit
+#pragma unroll
+        for (int r = 0; r < 2; ++r) {
+            float mx = m[r];
+#pragma unroll
+            for (int j = 0; j < 8; ++j)
+#pragma unroll
+                for (int e = 0; e < 2; ++e) {
+                    float &x = s[4 * j + 2 * r + e];
+                    x = (diag && j0 + 8 * j + fc + e > lim[r]) ? -INFINITY : x * kScale;
+                    mx = fmaxf(mx, x);
+                }
+            mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+            mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));  // finite: key 0 of tile 0 is in every row
+            const int prow = fr + 8 * r;
+            uint8_t *hrow = ph_sm + prow * 128, *lrow = pl_sm + prow * 128;
+            float sum = 0.f;
+#pragma unroll
+            for (int j = 0; j < 8; ++j) {
+                __align__(4) T hi[2], lo[2];
+#pragma unroll
+                for (int e = 0; e < 2; ++e) {
+                    const float pr = expf(s[4 * j + 2 * r + e] - mx);  // masked: exp(-inf) = 0
+                    hi[e] = from_f<T>(pr);
+                    lo[e] = from_f<T>(pr - to_f(hi[e]));
+                    sum += pr;
+                }
+                // K-major A operand, 128B swizzle: key c of row prow at 16-byte chunk (c / 8) ^ (prow % 8)
+                const int boff = (((j ^ (prow & 7)) << 4)) + 2 * fc;
+                *reinterpret_cast<uint32_t *>(hrow + boff) = *reinterpret_cast<const uint32_t *>(hi);
+                *reinterpret_cast<uint32_t *>(lrow + boff) = *reinterpret_cast<const uint32_t *>(lo);
+            }
+            sum += __shfl_xor_sync(0xffffffffu, sum, 1);
+            sum += __shfl_xor_sync(0xffffffffu, sum, 2);
+            const float corr = expf(m[r] - mx);  // m = -inf (first tile): 0, and o, l are still 0
+            l[r] = l[r] * corr + sum;
+            m[r] = mx;
+#pragma unroll
+            for (int g = 0; g < DG; ++g)
+#pragma unroll
+                for (int j = 0; j < 8; ++j) {
+                    o[g][4 * j + 2 * r] *= corr;
+                    o[g][4 * j + 2 * r + 1] *= corr;
+                }
+        }
+        fence_proxy_async();
+        __syncthreads();  // P complete (and the zeroed V rows visible to the tensor core)
+        wg_fence();
+#pragma unroll
+        for (int g = 0; g < DG; ++g) {
+            // B = V (MN-major): the [64 keys x 64 head columns] box g, 8-key groups 1 KB apart, one k16 step = 16 keys = 2 KB
+            const uint32_t vb = smem_u32(vs) + g * (PK_BK * 128);
+#pragma unroll
+            for (int kk = 0; kk < PK_BK / 16; ++kk)
+                Wgmma<T, 64>::template mma<0, 1>(o[g], gmma_desc_sw128(smem_u32(ph_sm) + kk * 32, 0, 1024),
+                                                 gmma_desc_sw128(vb + kk * 2048, PK_BK * 128, 1024), 1u);
+#pragma unroll
+            for (int kk = 0; kk < PK_BK / 16; ++kk)
+                Wgmma<T, 64>::template mma<0, 1>(o[g], gmma_desc_sw128(smem_u32(pl_sm) + kk * 32, 0, 1024),
+                                                 gmma_desc_sw128(vb + kk * 2048, PK_BK * 128, 1024), 1u);
+        }
+        wg_commit();
+        wg_wait<0>();
+        __syncthreads();  // P and this K / V stage are free again
+    }
+
+    T *obase = (T *)a.out + ((int64_t)bh * a.S + i0) * D;
+#pragma unroll
+    for (int r = 0; r < 2; ++r) {
+        const int row = fr + 8 * r;
+        if (i0 + row >= a.S) continue;
+        const float inv = 1.f / l[r];
+#pragma unroll
+        for (int g = 0; g < DG; ++g)
+#pragma unroll
+            for (int j = 0; j < 8; ++j) {
+                __align__(4) T ov[2] = {from_f<T>(o[g][4 * j + 2 * r] * inv), from_f<T>(o[g][4 * j + 2 * r + 1] * inv)};
+                *reinterpret_cast<uint32_t *>(obase + (int64_t)row * D + g * 64 + 8 * j + fc) = *reinterpret_cast<const uint32_t *>(ov);
+            }
+    }
+}
+
+template <typename T, int D>
+static int launch_prompt(void *kc, void *vc, const void *q, const void *k, const void *v, const PkArgs &a, int B,
+                         cudaStream_t st) {
+    const int64_t chunks = (int64_t)a.S * D / 8;
+    cudaError_t e = launch_k(kvcache_append_kernel<T>, dim3((unsigned)((chunks + 255) / 256), B * a.Hkv), dim3(256), (size_t)0, st,
+                             (T *)kc, (T *)vc, (const T *)k, (const T *)v, a.pos, a.pos_flags, a.Hkv, a.S, a.Smax, D);
+    ITB_CHECK(e == cudaSuccess, "AttentionKVCache prompt: append launch failed: %s", cudaGetErrorString(e));
+    CUtensorMap mq, mk, mv;
+    if (!make_tma_3d_b16(&mq, q, (uint64_t)B * a.Hq, (uint64_t)a.S, D, D, (uint64_t)a.S * D, PK_BQ, 64) ||
+        !make_tma_3d_b16(&mk, kc, (uint64_t)B * a.Hkv, (uint64_t)a.Smax, D, D, (uint64_t)a.Smax * D, PK_BK, 64) ||
+        !make_tma_3d_b16(&mv, vc, (uint64_t)B * a.Hkv, (uint64_t)a.Smax, D, D, (uint64_t)a.Smax * D, PK_BK, 64))
+        ITB_FAIL("AttentionKVCache prompt: cuTensorMapEncodeTiled failed");
+    const int smem = 5 * PK_BQ * D * 2 + 2 * PK_BQ * PK_BK * 2 + 1024;
+    auto kern = attention_kvcache_prompt_kernel<T, D>;
+    e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+    ITB_CHECK(e == cudaSuccess, "AttentionKVCache prompt: smem attribute: %s", cudaGetErrorString(e));
+    e = launch_k(kern, dim3((a.S + PK_BQ - 1) / PK_BQ, B * a.Hq), dim3(PK_THREADS), (size_t)smem, st, mq, mk, mv, a);
+    ITB_CHECK(e == cudaSuccess, "AttentionKVCache prompt: launch failed: %s", cudaGetErrorString(e));
+    ITB_LAUNCH_CHECK("AttentionKVCache prompt");
+    return 0;
+}
+
 }  // namespace itb
 
 using namespace itb;
@@ -472,4 +724,36 @@ extern "C" int it_b200_attention_prefill_strided(int dtype, const void *q, const
     if (dtype == ITB_BF16)
         return D == 64 ? launch_ap<__nv_bfloat16, 64>(q, k, v, a, st, &sq, &sk, &sv) : launch_ap<__nv_bfloat16, 128>(q, k, v, a, st, &sq, &sk, &sv);
     return D == 64 ? launch_ap<__half, 64>(q, k, v, a, st, &sq, &sk, &sv) : launch_ap<__half, 128>(q, k, v, a, st, &sq, &sk, &sv);
+}
+
+// AttentionKVCache over S >= 1 new tokens per batch row (S = 1 is one decode step, served by the same two launches)
+extern "C" int it_b200_attention_kvcache_prompt(int dtype, void *k_cache, void *v_cache, const void *q, const void *k,
+                                                const void *v, const void *position_id, int pos_flags, void *out, int B,
+                                                int Hq, int Hkv, int S, int S_max, int D, void *stream) {
+    ITB_CHECK(dtype == ITB_F16 || dtype == ITB_BF16, "AttentionKVCache prompt: dtype %d must be f16 / bf16 (no fp32 prefill)", dtype);
+    ITB_CHECK(D == 64 || D == 128, "AttentionKVCache prompt: head dim %d must be 64 or 128", D);
+    const int pos_dtype = pos_flags & 0xff;
+    ITB_CHECK(pos_dtype == ITB_I32 || pos_dtype == ITB_U32 || pos_dtype == ITB_I64,
+              "AttentionKVCache prompt: position dtype %d must be int32/uint32/int64", pos_dtype);
+    ITB_CHECK(B >= 0 && Hq >= 0 && S >= 1 && S <= S_max, "AttentionKVCache prompt: %d tokens do not fit a cache of %d rows", S, S_max);
+    ITB_CHECK(Hkv > 0 && Hq % Hkv == 0, "AttentionKVCache prompt: %d query heads are not a multiple of %d KV heads", Hq, Hkv);
+    ITB_CHECK((int64_t)B * Hq <= 65535 && (int64_t)B * Hkv <= 65535, "AttentionKVCache prompt: batch x heads beyond the grid limit");
+    if ((int64_t)B * Hq == 0) return 0;
+    ITB_CHECK(aligned16(k_cache) && aligned16(v_cache) && aligned16(q) && aligned16(k) && aligned16(v) && aligned16(out),
+              "AttentionKVCache prompt: tensors must be 16-byte aligned");
+    PkArgs a{};
+    a.pos = position_id;
+    a.pos_flags = pos_flags;
+    a.out = out;
+    a.Hq = Hq;
+    a.Hkv = Hkv;
+    a.G = Hq / Hkv;
+    a.S = S;
+    a.Smax = S_max;
+    auto st = (cudaStream_t)stream;
+    if (dtype == ITB_BF16)
+        return D == 64 ? launch_prompt<__nv_bfloat16, 64>(k_cache, v_cache, q, k, v, a, B, st)
+                       : launch_prompt<__nv_bfloat16, 128>(k_cache, v_cache, q, k, v, a, B, st);
+    return D == 64 ? launch_prompt<__half, 64>(k_cache, v_cache, q, k, v, a, B, st)
+                   : launch_prompt<__half, 128>(k_cache, v_cache, q, k, v, a, B, st);
 }

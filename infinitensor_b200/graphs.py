@@ -128,13 +128,17 @@ class LlamaGraph:
     weights: dict = field(default_factory=dict)  # name -> (tensor, shape, kind, shard)
 
 
-def build_llama_decode(h, cfg: LlamaConfig, world: int = 1, rank: int = 0) -> LlamaGraph:
-    """One decode step.  world > 1 applies the reference's tensor-parallel cut (parallel_opt.py):
+def build_llama_decode(h, cfg: LlamaConfig, world: int = 1, rank: int = 0, seq: int = 1) -> LlamaGraph:
+    """One decode step, or with seq > 1 one prompt step: seq new tokens per batch row at positions p_b .. p_b + seq - 1
+    (input_ids and position_ids [B, seq], logits [B, seq, vocab]; AttentionKVCache appends all of them and attends
+    causally).  world > 1 applies the reference's tensor-parallel cut (parallel_opt.py):
     q/k/v + gate/up column-split, o/down row-split followed by AllReduceSum, KV cache split by head,
     embedding / norms / logits replicated.  cfg.kv_heads < cfg.heads builds grouped-query attention: k / v projections
     and caches carry the KV heads, query head i reads KV head i // (heads // kv_heads)."""
     assert cfg.heads % world == 0 and cfg.ffn % world == 0
     assert cfg.n_kv % world == 0 and cfg.heads % cfg.n_kv == 0
+    # the FP8 weight GEMM takes at most 64 rows, and a tensor-parallel prompt step is not provided
+    assert seq == 1 or (world == 1 and not cfg.fp8_weights), "prompt steps (seq > 1): one GPU, 16-bit weights"
     B, d, H, dh, f, V, dt = cfg.batch, cfg.d_model, cfg.heads // world, cfg.head_dim, cfg.ffn // world, cfg.vocab, cfg.dtype
     Hkv = cfg.n_kv // world
     dl, dkv = H * dh, Hkv * dh  # local attention widths of q and of k / v
@@ -161,12 +165,12 @@ def build_llama_decode(h, cfg: LlamaConfig, world: int = 1, rank: int = 0) -> Ll
         g.weights[name + ".scale"] = (sc, (shape[1],), "scale", None)
         return h.matmul(x_, wq, None, False, False, None, LINEAR, w_scale=sc)
 
-    g.input_ids = h.tensor([B, 1], I64)
-    g.position_ids = h.tensor([B, 1], I64)
+    g.input_ids = h.tensor([B, seq], I64)
+    g.position_ids = h.tensor([B, seq], I64)
     g.input_ids.set_input()
     g.position_ids.set_input()
     emb = weight("embed", (V, d), "embed")
-    x = h.gather(emb, g.input_ids, None, 0)  # [B,1,d]
+    x = h.gather(emb, g.input_ids, None, 0)  # [B,seq,d]
     for li in range(cfg.layers):
         p = f"l{li}."
         kc = h.tensor([B, Hkv, cfg.s_max, dh], dt)
@@ -183,11 +187,11 @@ def build_llama_decode(h, cfg: LlamaConfig, world: int = 1, rank: int = 0) -> Ll
         k = h.RoPE(g.position_ids, k, None, **rope_kw)
 
         def heads(t, n=H):
-            t = h.reshape(t, None, [B, 1, n, dh])
-            return h.transpose(t, None, [0, 2, 1, 3])  # [B,n,1,dh]
+            t = h.reshape(t, None, [B, seq, n, dh])
+            return h.transpose(t, None, [0, 2, 1, 3])  # [B,n,seq,dh]
 
         attn = h.attentionKVCache(kc, vc, heads(q), heads(k, Hkv), heads(v, Hkv), g.position_ids, None)
-        a = h.reshape(h.transpose(attn, None, [0, 2, 1, 3]), None, [B, 1, dl])
+        a = h.reshape(h.transpose(attn, None, [0, 2, 1, 3]), None, [B, seq, dl])
         o = linear(a, p + "wo", (dl, d), ("row", d))
         if world > 1:
             o = h.allReduceSum(o, None)
