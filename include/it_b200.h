@@ -318,6 +318,20 @@ int it_b200_attention_kvcache_gqa(int dtype, void *k_cache, void *v_cache, const
                                   int B, int Hq, int Hkv, int S_max, int D, void *workspace, int64_t workspace_bytes,
                                   void *stream);
 
+/* ---- AttentionKVCache (decode, one token per step) over an FP8 E4M3 KV cache: it_b200_attention_kvcache_gqa with caches
+ *      [B,Hkv,S_max,D] of one-byte OCP E4M3 "FN" codes and k_scale / v_scale, f32 [Hkv], one scale per KV head.  A cache
+ *      element's value is e4m3(code) * scale[h].  dtype (q / k / v / out) is ITB_F16 or ITB_BF16; fp32 is refused.
+ *      Append: row p of KV head h is stored as code = cvt.rn.satfinite.e4m3(fp32(x) / scale[h]) -- the fp32 division correctly
+ *      rounded, round to nearest even, saturated to +-448 -- with k rotated first (in the activation type) when rope_pos is
+ *      given.  Attention over rows 0 .. p, the appended row read back from its codes:
+ *        s_j = fp32(q . code_k,j) * scale_k[h] / sqrt(D),  stable softmax,  out = (sum_j p_j code_v,j) / l * scale_v[h] rounded
+ *      once to the activation type (codes widen exactly to f16 / bf16).  Positions, pos_flags, RoPE, G = Hq / Hkv and the
+ *      workspace (it_b200_attention_kvcache_workspace(B, Hq, S_max, D)) are as for it_b200_attention_kvcache_gqa. ---- */
+int it_b200_attention_kvcache_fp8(int dtype, void *k_cache, void *v_cache, const void *k_scale, const void *v_scale,
+                                  const void *q, const void *k, const void *v, const void *position_id, int pos_flags,
+                                  const void *rope_pos, int rope_pos_dtype, void *out, int B, int Hq, int Hkv, int S_max,
+                                  int D, void *workspace, int64_t workspace_bytes, void *stream);
+
 /* ---- AttentionKVCache over a prompt chunk of S >= 1 new tokens (attention_prefill.cu): exactly S single-token AttentionKVCache
  *      calls in order, token i of batch row b at position p_b + i.  Caches [B,Hkv,S_max,D]; q / out [B,Hq,S,D]; k / v [B,Hkv,S,D];
  *      Hq = G * Hkv.  Token i's k / v are copied into cache row p_b + i; query i of head h attends over rows 0 .. p_b + i of KV

@@ -85,6 +85,8 @@ _SIGS = {
                                           vp, c_int64, vp]),
     "it_b200_attention_kvcache_gqa": (c_int, [c_int, vp, vp, vp, vp, vp, vp, c_int, vp, c_int, vp, c_int, c_int, c_int, c_int,
                                               c_int, vp, c_int64, vp]),
+    "it_b200_attention_kvcache_fp8": (c_int, [c_int, vp, vp, vp, vp, vp, vp, vp, vp, c_int, vp, c_int, vp, c_int, c_int, c_int,
+                                              c_int, c_int, vp, c_int64, vp]),
     "it_b200_attention_kvcache_prompt": (c_int, [c_int, vp, vp, vp, vp, vp, vp, c_int, vp] + [c_int] * 6 + [vp]),
     "it_b200_attention_prefill": (c_int, [c_int, vp, vp, vp, vp, c_int, c_int, c_int, c_int, c_int, vp, c_int, vp, c_int64, c_int64,
                                           c_int64, c_int64, vp]),

@@ -529,6 +529,12 @@ void runAttentionRope(const Operator &ropeQ, const Operator &ropeK, const Operat
     const int hq = att->getInputs(2)->getDims()[1];  // = G x the caches' d[1] KV heads
     int64_t wsb = it_b200_attention_kvcache_workspace(d[0], hq, d[2], d[3]);
     void *ws = wsb ? RT(ctx)->getWorkspace((size_t)wsb) : nullptr;
+    if (as<AttentionKVCacheObj>(att)->isFp8Cache()) {  // FP8 E4M3 caches + per-KV-head scales
+        CK(it_b200_attention_kvcache_fp8(DTI(qpre), P(kc), P(vc), P(att->getInputs(6)), P(att->getInputs(7)), P(qpre), P(kpre), P(v),
+                                         P(pos), attnPosFlags(att, rpos), P(rpos), DTI(rpos), P(att->getOutput()), d[0], hq, d[1],
+                                         d[2], d[3], ws, wsb, S()), att);
+        return;
+    }
     CK(it_b200_attention_kvcache_gqa(DTI(qpre), P(kc), P(vc), P(qpre), P(kpre), P(v), P(pos), attnPosFlags(att, rpos), P(rpos),
                                      DTI(rpos), P(att->getOutput()), d[0], hq, d[1], d[2], d[3], ws, wsb, S()), att);
 }
@@ -784,6 +790,14 @@ class AttentionKVCacheB200 : public CudaKernelWithoutConfig {
         }
         int64_t wsb = it_b200_attention_kvcache_workspace(d[0], hq, d[2], d[3]);
         void *ws = wsb ? RT(ctx)->getWorkspace((size_t)wsb) : nullptr;
+#ifndef ITB_SEAM_A
+        if (kc->getDType() == DataType::Float8E4M3FN) {  // FP8 E4M3 caches + per-KV-head scales (inputs 6, 7)
+            CK(it_b200_attention_kvcache_fp8(DTI(q), P(kc), P(vc), P(op->getInputs(6)), P(op->getInputs(7)), P(q), P(k), P(v), P(pos),
+                                             b200::attnPosFlags(op, nullptr), nullptr, 0, P(op->getOutput()), d[0], hq, d[1], d[2],
+                                             d[3], ws, wsb, S()), op);
+            return;
+        }
+#endif
         CK(it_b200_attention_kvcache_gqa(DTI(q), P(kc), P(vc), P(q), P(k), P(v), P(pos),
 #ifdef ITB_SEAM_A
                                          DTI(pos) | (pos->getSource() || kc->getSource() || vc->getSource() ? ITB_POS_IN_STEP : 0),

@@ -80,16 +80,40 @@ vector<int> ConvObj::getWorkloadVector() const {
 }
 
 // ---------------------------------------------------------------- AttentionKVCache (attention_kvcache.cc:5-27)
+static TensorVec attentionInputs(TensorVec v, Tensor kScale, Tensor vScale) {
+    IT_ASSERT(!kScale == !vScale, "AttentionKVCache: k_scale and v_scale go together");
+    if (kScale) {
+        v.push_back(kScale);
+        v.push_back(vScale);
+    }
+    return v;
+}
 AttentionKVCacheObj::AttentionKVCacheObj(GraphObj *graph, Tensor input_k_cache, Tensor input_v_cache,
                                          Tensor input_q, Tensor input_k, Tensor input_v, Tensor position_id,
-                                         Tensor output_matmul, bool perRowPositions)
-    : OperatorObj(OpType::AttentionKVCache, {input_k_cache, input_v_cache, input_q, input_k, input_v, position_id},
+                                         Tensor output_matmul, bool perRowPositions, Tensor k_scale, Tensor v_scale)
+    : OperatorObj(OpType::AttentionKVCache,
+                  attentionInputs({input_k_cache, input_v_cache, input_q, input_k, input_v, position_id}, k_scale, v_scale),
                   {output_matmul}),
       perRowPositions(perRowPositions) {
     IT_ASSERT(checkValid(graph));
 }
 std::optional<vector<Shape>> AttentionKVCacheObj::inferShape(const TensorVec &ins) {
-    IT_ASSERT(ins.size() == 6);
+    IT_ASSERT(ins.size() == 6 || ins.size() == 8, "AttentionKVCache takes 6 inputs, or 8 with an FP8 cache's scales");
+    const bool fp8k = ins[0]->getDType() == DataType::Float8E4M3FN, fp8v = ins[1]->getDType() == DataType::Float8E4M3FN;
+    // FP8 E4M3 caches (extension): k_scale / v_scale f32 [Hkv] are inputs 6 and 7, present exactly when the caches are FP8
+    IT_ASSERT(fp8k == fp8v, "AttentionKVCache: k_cache and v_cache must both be FP8 or neither");
+    IT_ASSERT(fp8k == (ins.size() == 8), fp8k ? "AttentionKVCache: an FP8 KV cache needs k_scale and v_scale"
+                                              : "AttentionKVCache: k_scale / v_scale go with FP8 caches only");
+    if (fp8k) {
+        for (int i : {6, 7})
+            IT_ASSERT(ins[i]->getDType() == DataType::Float32 && ins[i]->getRank() == 1 && ins[0]->getRank() == 4 &&
+                          ins[i]->getDims()[0] == ins[0]->getDims()[1],
+                      "AttentionKVCache: k_scale / v_scale must be f32 [Hkv], one scale per KV head");
+        for (int i : {2, 3, 4})
+            IT_ASSERT(ins[i]->getDType() == DataType::Float16 || ins[i]->getDType() == DataType::BFloat16,
+                      "AttentionKVCache: an FP8 KV cache takes f16 / bf16 q, k and v");
+        IT_ASSERT(ins[2]->getRank() == 4 && ins[2]->getDims()[2] == 1, "AttentionKVCache: an FP8 KV cache takes one token per step");
+    }
     IT_ASSERT(ins[0]->getRank() == 4 && ins[2]->getRank() == 4, "AttentionKVCache expects rank-4 tensors");
     IT_ASSERT(ins[0]->getDims() == ins[1]->getDims(), "k_cache / v_cache shapes differ");
     IT_ASSERT(ins[3]->getDims() == ins[4]->getDims(), "k / v shapes differ");

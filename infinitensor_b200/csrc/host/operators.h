@@ -67,10 +67,12 @@ class AttentionKVCacheObj : public OperatorObj {
     bool perRowPositions;  // extension (SURVEY 8(f-3)): row b attends up to position_id[b]; false = the reference's element-0 rule
 
   public:
+    // k_scale / v_scale (extension): the caches hold FP8 E4M3 codes, element value e4m3(code) * scale[KV head]; f32 [Hkv]
     AttentionKVCacheObj(GraphObj *graph, Tensor input_k_cache, Tensor input_v_cache, Tensor input_q,
                         Tensor input_k, Tensor input_v, Tensor position_id, Tensor output_matmul,
-                        bool perRowPositions = false);
+                        bool perRowPositions = false, Tensor k_scale = nullptr, Tensor v_scale = nullptr);
     bool getPerRowPositions() const { return perRowPositions; }
+    bool isFp8Cache() const { return inputs.size() == 8; }
     vector<int> getOpAttrVector() const override { return {(int)type.underlying(), (int)perRowPositions}; }
     std::optional<vector<Shape>> inferShape(const TensorVec &inputs) override;
     vector<DataType> inferDataType(const TensorVec &ins) const override { return {ins[2]->getDType()}; }

@@ -18,6 +18,7 @@
 // 2*U 16-byte requests in flight.
 #include <algorithm>
 #include <string>
+#include <type_traits>
 
 #include "common.cuh"
 #include "gemm.cuh"  // mbarrier / bulk-copy PTX helpers
@@ -72,6 +73,31 @@ __device__ __forceinline__ void rope_one(Vec16<T> &x, int col, const float *cs_t
         const float a = round_t<T>(__fmul_rn(to_f(x.v[j]), cs_t[c])), b = round_t<T>(__fmul_rn(to_f(xp.v[j]), sn_t[c]));
         x.v[j] = from_f<T>(lo ? a - b : a + b);
     }
+}
+
+// FP8 E4M3 KV cache (cache element type uint8_t; an element's value is e4m3(code) * scale[KV head]).  Every E4M3 value is exact
+// in f16, so codes widen through cvt.rn.f16x2.e4m3x2 with no loss, for bf16 activations too; scales enter only in fp32.
+// 16 codes (one 16-byte load) -> 16 fp32 values
+__device__ __forceinline__ void e4m3x16_to_f(const uint4 raw, float (&f)[16]) {
+    const uint32_t w[4] = {raw.x, raw.y, raw.z, raw.w};
+#pragma unroll
+    for (int i = 0; i < 4; ++i)
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            const uint32_t h2 = e4m3x2_to<__half>(w[i] >> (16 * h));
+            const float2 x = __half22float2(*reinterpret_cast<const __half2 *>(&h2));
+            f[4 * i + 2 * h] = x.x;
+            f[4 * i + 2 * h + 1] = x.y;
+        }
+}
+// the append's quantiser: code = cvt.rn.satfinite.e4m3(fp32(x) / scale), the division correctly rounded (not a multiply by a
+// reciprocal), so that a host restatement matches it bit for bit
+template <typename T> __device__ __forceinline__ uint2 quantise_e4m3x8(const Vec16<T> &x, float scale) {
+    uint32_t c[4];
+#pragma unroll
+    for (int i = 0; i < 4; ++i)
+        c[i] = f32x2_to_e4m3x2(__fdiv_rn(to_f(x.v[2 * i]), scale), __fdiv_rn(to_f(x.v[2 * i + 1]), scale));
+    return make_uint2(c[0] | (c[1] << 16), c[2] | (c[3] << 16));
 }
 
 constexpr int AS_MAX_B = 1024;  // batch rows whose (position, chunk count) the CTA keeps in shared memory
@@ -435,8 +461,9 @@ __device__ __forceinline__ void
 // ------------------------------------------------------------------------------------------------------------------
 constexpr int GQ_WARPS = 8;
 
-template <typename T, int D> struct GqaCfg {
-    static constexpr int CH = 16384 / (D * (int)sizeof(T));  // cache rows per 16 KiB chunk: 64 / 128 (f16 / bf16), 32 / 64 (fp32)
+template <typename T, int D, typename KT = T> struct GqaCfg {  // KT: the cache element type
+    static constexpr int CH = 16384 / (D * (int)sizeof(KT));  // cache rows per 16 KiB chunk: 64 / 128 (f16 / bf16), 32 / 64 (fp32),
+                                                              // 128 / 256 (FP8)
     static constexpr int NC = CH / (GQ_WARPS * 4);           // S columns per thread: 2 / 4, 1 / 2
     static constexpr int NT = NC / 2;                        // f16 / bf16: n8 tiles of S per warp
     static constexpr int NJ = D / (8 * GQ_WARPS);            // n8 tiles of O per warp
@@ -885,6 +912,783 @@ __device__ __forceinline__ void
     }
 }
 
+// ------------------------------------------------------------------------------------------------------------------
+// attn_stream_kv8_kernel: attn_stream_kernel over an FP8 E4M3 cache (uint8_t codes, one fp32 scale per head in k_scale /
+// v_scale).  Same dealing, ring, tickets, merge and workspace; a lane holds 16 codes of a row (one 16-byte load) and widens
+// them in registers before the fp32 dot products, so a 16 KiB chunk holds twice the rows of a 16-bit one and the ring's
+// bytes in flight are unchanged.  K's scale folds into q with 1/sqrt(D); V's scales the normalised output once.
+// ------------------------------------------------------------------------------------------------------------------
+template <typename T, int D, int WARPS, int U, bool ROPE>
+__device__ __forceinline__ void
+    attn_stream_kv8_body(uint8_t *__restrict__ kcache, uint8_t *__restrict__ vcache, const T *__restrict__ q,
+                       const T *__restrict__ kin, const T *__restrict__ vin, const void *__restrict__ position_id,
+                       int pos_flags, T *__restrict__ out, int Smax, int BH, float *__restrict__ partial,
+                       int slots_per_head, int *__restrict__ tickets, const void *__restrict__ rope_pos,
+                       int rope_pos_dtype, int H, const float *__restrict__ k_scale, const float *__restrict__ v_scale) {
+    using KT = uint8_t;
+    using C = RowCfg<KT, D>;
+    constexpr int EPL = C::EPL, LPR = C::LPR, RPW = C::RPW;
+    constexpr int CH = WARPS * RPW * U;                       // cache rows per chunk
+    constexpr int CHUNK_BYTES = CH * D * (int)sizeof(KT);     // 16 KiB for every dtype and width
+    constexpr int CONSUMERS = WARPS * 32;
+    extern __shared__ __align__(128) unsigned char ring[];    // stages x { K chunk | V chunk }
+    __shared__ __align__(8) uint64_t full[AS_STAGES], empty[AS_STAGES];
+    __shared__ float s_m[WARPS], s_l[WARPS];
+    __shared__ float s_acc[WARPS][D];
+    __shared__ float s_cs[D / 2], s_sn[D / 2];
+    __shared__ int s_last;
+    __shared__ int s_pos[AS_MAX_B];       // clamped position of batch row b
+    __shared__ int s_pre[AS_MAX_B + 1];   // (head, chunk) units before batch row b; s_pre[B] = total
+
+    pdl_trigger();
+    const int pos_dtype = pos_flags & 0xff;
+    const bool per_row = (pos_flags & ITB_POS_PER_ROW) != 0;
+    // ITB_POS_IN_STEP: the position tensor / RoPE positions / cache rows below the position may have been written by a
+    // kernel of THIS step (an ONNX graph that computes position_ids or concatenates the past in-graph): nothing is read
+    // ahead of griddepcontrol.wait.  Otherwise they are a whole step old (graph inputs, the previous step's appends) and
+    // the producer starts streaming while the previous kernel of the chain drains.
+    if (pos_flags & ITB_POS_IN_STEP) pdl_wait();
+    const int Bn = BH / H;
+    if (threadIdx.x == 0) {
+        for (int s = 0; s < AS_STAGES; ++s) {
+            mbar_init(&full[s], 1);
+            mbar_init(&empty[s], WARPS);
+        }
+        fence_mbar_init();
+    }
+    for (int b = threadIdx.x; b < Bn; b += blockDim.x) {
+        int p = pos_dtype == ITB_I64 ? read_pos<int64_t>(position_id, per_row ? b : 0)
+                                     : read_pos<int32_t>(position_id, per_row ? b : 0);
+        s_pos[b] = min(max(p, 0), Smax - 1);
+    }
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        int acc = 0;
+        for (int b = 0; b < Bn; ++b) {
+            s_pre[b] = acc;
+            acc += H * (s_pos[b] / CH + 1);  // chunks per head of row b; the last one holds rows [.., pos) + the appended row
+        }
+        s_pre[Bn] = acc;
+    }
+    __syncthreads();
+    // Everything this step produced (q, k, v) is read by the consumers, after their wait; this kernel's own append
+    // touches row `pos` only, which the bulk loads never include.
+
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int64_t total = s_pre[Bn], G = min((int64_t)gridDim.x, total);
+    // this CTA's contiguous range of (head, chunk) units: [u0, u0 + nunits), starting at (bh, c) inside batch row b.
+    // G = CTAs that take part: never more than there are units, so every one owns >= 1 unit and the CTAs sharing a head
+    // are consecutive
+    if (blockIdx.x >= G) return;
+    int nunits, bh, c, brow, pos, nch;
+    {
+        const int64_t u0 = blockIdx.x * total / G, u1 = (blockIdx.x + 1) * total / G;
+        nunits = (int)(u1 - u0);
+        brow = 0;
+        while (brow + 1 < Bn && s_pre[brow + 1] <= u0) ++brow;
+        pos = s_pos[brow];
+        nch = pos / CH + 1;
+        const int r = (int)(u0 - s_pre[brow]);
+        bh = brow * H + r / nch;
+        c = r % nch;
+    }
+    auto next_unit = [&]() {  // (bh, c) -> the next unit; entering a new batch row refreshes its position
+        if (++c == nch) {
+            c = 0;
+            ++bh;
+            if (bh % H == 0 && bh < BH) {
+                brow = bh / H;
+                pos = s_pos[brow];
+                nch = pos / CH + 1;
+            }
+        }
+    };
+
+    if (warp == WARPS) {
+        // ---------------- producer: one elected lane streams chunks into the ring ----------------
+        if (lane == 0) {
+            const uint64_t policy = l2_policy_evict_first();
+            int st = 0, ph = 0;
+            for (int it = 0; it < nunits; ++it) {
+                mbar_wait(&empty[st], ph ^ 1);
+                const int rows = min(CH, pos - c * CH);
+                if (rows > 0) {
+                    const uint32_t bytes = (uint32_t)rows * D * (uint32_t)sizeof(KT);
+                    const int64_t off = ((int64_t)bh * Smax + (int64_t)c * CH) * D;
+                    mbar_expect_tx(&full[st], 2 * bytes);
+                    bulk_load_1d(ring + (size_t)st * 2 * CHUNK_BYTES, kcache + off, bytes, &full[st], policy);
+                    bulk_load_1d(ring + (size_t)st * 2 * CHUNK_BYTES + CHUNK_BYTES, vcache + off, bytes, &full[st], policy);
+                } else {
+                    mbar_arrive(&full[st]);
+                }
+                next_unit();
+                if (++st == AS_STAGES) { st = 0; ph ^= 1; }
+            }
+        }
+        return;
+    }
+
+    // ---------------- consumers ----------------
+    // RoPE cos / sin table of the CTA's first batch row: the RoPE positions are a step-old graph input like the cache
+    // position, so the powf / sincosf chain runs ahead of the wait; recomputed only when a later segment changes batch row
+    int table_b = -1;
+    auto rope_table = [&](int b) {
+        if (threadIdx.x < D / 2) {
+            const float p = rope_pos_dtype == ITB_I64 ? (float)(int)((const int64_t *)rope_pos)[b]
+                                                      : (float)((const int32_t *)rope_pos)[b];
+            const float freq = p * powf(10000.f, -(float)(threadIdx.x * 2) / (float)D);
+            s_cs[threadIdx.x] = round_t<T>(cosf(freq));
+            s_sn[threadIdx.x] = round_t<T>(sinf(freq));
+        }
+        named_bar_sync(1, CONSUMERS);
+        table_b = b;
+    };
+    if (ROPE) rope_table(bh / H);
+    pdl_wait();  // (a no-op the second time under ITB_POS_IN_STEP)
+    const int sub = lane / LPR;
+    const int col = (lane % LPR) * EPL;
+    float qf[EPL], m = -INFINITY, l = 0.f, acc[EPL];
+    bool seg_from_start = false;
+    int st = 0, ph = 0;
+    for (int it = 0; it < nunits; ++it) {
+        if (it == 0 || c == 0) {
+            // new head segment: reset the running softmax, fetch (and rotate) q
+            seg_from_start = c == 0;
+            m = -INFINITY;
+            l = 0.f;
+#pragma unroll
+            for (int j = 0; j < EPL; ++j) acc[j] = 0.f;
+            // 16 columns per lane: two 8-wide halves
+            Vec16<T> qa = ld16(q + (int64_t)bh * D + col), qb = ld16(q + (int64_t)bh * D + col + 8);
+            if (ROPE) {
+                if (bh / H != table_b) rope_table(bh / H);
+                rope_one<T, D, 8, LPR>(qa, col, s_cs, s_sn);
+                rope_one<T, D, 8, LPR>(qb, col + 8, s_cs, s_sn);
+            }
+            const float qs = k_scale[bh % H] * attn_scale<D>();
+#pragma unroll
+            for (int j = 0; j < 8; ++j) {
+                qf[j] = to_f(qa.v[j]) * qs;
+                qf[8 + j] = to_f(qb.v[j]) * qs;
+            }
+        }
+        const int nvalid = pos - c * CH;  // cache rows of this chunk that exist (<= 0: only the appended row)
+        const unsigned char *kb = ring + (size_t)st * 2 * CHUNK_BYTES, *vb = kb + CHUNK_BYTES;
+        mbar_wait(&full[st], ph);
+#ifndef ATTN_DBG_NOCOMPUTE  // (debug builds only: measures the bare HBM -> smem ring)
+        const KT *ks = reinterpret_cast<const KT *>(kb) + (warp * U * RPW + sub) * D + col;
+        const KT *vs = reinterpret_cast<const KT *>(vb) + (warp * U * RPW + sub) * D + col;
+        if (nvalid >= CH) {
+            // full chunk (every chunk but a head's last): branch-free, so the U rows' load / dot / shuffle chains interleave
+            float sc[U];
+#pragma unroll
+            for (int uu = 0; uu < U; ++uu) {
+                float kf[EPL];
+                e4m3x16_to_f(*reinterpret_cast<const uint4 *>(ks + uu * RPW * D), kf);
+                float d = 0.f;
+#pragma unroll
+                for (int j = 0; j < EPL; ++j) d += qf[j] * kf[j];
+                sc[uu] = d;
+            }
+#pragma unroll
+            for (int o = LPR / 2; o > 0; o >>= 1) {
+#pragma unroll
+                for (int uu = 0; uu < U; ++uu) sc[uu] += __shfl_xor_sync(0xffffffffu, sc[uu], o);
+            }
+            float mx = m;
+#pragma unroll
+            for (int uu = 0; uu < U; ++uu) mx = fmaxf(mx, sc[uu]);
+            const float corr = expf(m - mx);  // m = -inf -> 0
+            l *= corr;
+#pragma unroll
+            for (int j = 0; j < EPL; ++j) acc[j] *= corr;
+#pragma unroll
+            for (int uu = 0; uu < U; ++uu) {
+                float vf[EPL];
+                e4m3x16_to_f(*reinterpret_cast<const uint4 *>(vs + uu * RPW * D), vf);
+                const float p = expf(sc[uu] - mx);
+                l += p;
+#pragma unroll
+                for (int j = 0; j < EPL; ++j) acc[j] = fmaf(p, vf[j], acc[j]);
+            }
+            m = mx;
+        } else {
+            float sc[U];
+            bool ok[U];
+#pragma unroll
+            for (int uu = 0; uu < U; ++uu) {
+                ok[uu] = (warp * U + uu) * RPW + sub < nvalid;
+                float d = 0.f;
+                if (ok[uu]) {
+                    float kf[EPL];
+                    e4m3x16_to_f(*reinterpret_cast<const uint4 *>(ks + uu * RPW * D), kf);
+#pragma unroll
+                    for (int j = 0; j < EPL; ++j) d += qf[j] * kf[j];
+                }
+#pragma unroll
+                for (int o = LPR / 2; o > 0; o >>= 1) d += __shfl_xor_sync(0xffffffffu, d, o);
+                sc[uu] = ok[uu] ? d : -INFINITY;
+            }
+            float mx = m;
+#pragma unroll
+            for (int uu = 0; uu < U; ++uu) mx = fmaxf(mx, sc[uu]);
+            if (mx > -INFINITY) {
+                const float corr = expf(m - mx);  // m = -inf -> 0
+                l *= corr;
+#pragma unroll
+                for (int j = 0; j < EPL; ++j) acc[j] *= corr;
+#pragma unroll
+                for (int uu = 0; uu < U; ++uu) {
+                    if (ok[uu]) {
+                        float vf[EPL];
+                        e4m3x16_to_f(*reinterpret_cast<const uint4 *>(vs + uu * RPW * D), vf);
+                        const float p = expf(sc[uu] - mx);
+                        l += p;
+#pragma unroll
+                        for (int j = 0; j < EPL; ++j) acc[j] = fmaf(p, vf[j], acc[j]);
+                    }
+                }
+                m = mx;
+            }
+        }
+#endif
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&empty[st]);  // this warp is done with the stage
+        if (++st == AS_STAGES) { st = 0; ph ^= 1; }
+
+        const bool last_chunk = c == nch - 1;
+        if (last_chunk && warp == 0) {
+          // FP8: the appended row is quantised in registers, stored as codes, and contributes through its dequantised codes
+          const int64_t src = (int64_t)bh * D + col, dst = ((int64_t)bh * Smax + pos) * D + col;
+          Vec16<T> ka = ld16(kin + src), kb2 = ld16(kin + src + 8);
+          if (ROPE) {
+              rope_one<T, D, 8, LPR>(ka, col, s_cs, s_sn);
+              rope_one<T, D, 8, LPR>(kb2, col + 8, s_cs, s_sn);
+          }
+          const float ksc = k_scale[bh % H];
+          const uint2 k0 = quantise_e4m3x8(ka, ksc), k1 = quantise_e4m3x8(kb2, ksc);
+          const uint4 kcodes = make_uint4(k0.x, k0.y, k1.x, k1.y);
+          float kf[EPL];
+          e4m3x16_to_f(kcodes, kf);
+          float d = 0.f;
+  #pragma unroll
+          for (int j = 0; j < EPL; ++j) d += qf[j] * kf[j];
+  #pragma unroll
+          for (int o = LPR / 2; o > 0; o >>= 1) d += __shfl_xor_sync(0xffffffffu, d, o);
+          if (sub == 0) {
+              const float vs8 = v_scale[bh % H];
+              const uint2 v0 = quantise_e4m3x8(ld16(vin + src), vs8), v1 = quantise_e4m3x8(ld16(vin + src + 8), vs8);
+              const uint4 vcodes = make_uint4(v0.x, v0.y, v1.x, v1.y);
+              *reinterpret_cast<uint4 *>(kcache + dst) = kcodes;
+              *reinterpret_cast<uint4 *>(vcache + dst) = vcodes;
+              float vf[EPL];
+              e4m3x16_to_f(vcodes, vf);
+              const float mx2 = fmaxf(m, d);
+              const float corr = expf(m - mx2), pnew = expf(d - mx2);
+              l = l * corr + pnew;
+  #pragma unroll
+              for (int j = 0; j < EPL; ++j) acc[j] = fmaf(pnew, vf[j], acc[j] * corr);
+              m = mx2;
+          }
+        }
+        if (last_chunk || it == nunits - 1) {
+            // ---- segment end: fold sub-rows, warps, and (when the head is shared between CTAs) the other CTAs' partials
+#pragma unroll
+            for (int o = LPR; o < 32; o <<= 1) {
+                const float m2 = __shfl_xor_sync(0xffffffffu, m, o);
+                const float l2 = __shfl_xor_sync(0xffffffffu, l, o);
+                const float mm = fmaxf(m, m2);
+                const float c1 = mm > -INFINITY ? expf(m - mm) : 0.f, c2 = mm > -INFINITY ? expf(m2 - mm) : 0.f;
+                l = l * c1 + l2 * c2;
+#pragma unroll
+                for (int j = 0; j < EPL; ++j) {
+                    const float a2 = __shfl_xor_sync(0xffffffffu, acc[j], o);
+                    acc[j] = acc[j] * c1 + a2 * c2;
+                }
+                m = mm;
+            }
+            if (sub == 0) {
+#pragma unroll
+                for (int j = 0; j < EPL; ++j) s_acc[warp][col + j] = acc[j];
+                if (lane == 0) {
+                    s_m[warp] = m;
+                    s_l[warp] = l;
+                }
+            }
+            named_bar_sync(1, CONSUMERS);
+            const bool whole = seg_from_start && last_chunk;
+            // which CTAs share this head:  cta(u) = floor(((u + 1) G - 1) / total)
+            const int64_t hu0 = (int64_t)s_pre[brow] + (int64_t)(bh - brow * H) * nch;  // first unit of this head
+            const int first_cta = (int)(((hu0 + 1) * G - 1) / total);
+            const int last_cta = (int)(((hu0 + nch) * G - 1) / total);
+            const int nseg = last_cta - first_cta + 1;
+            float *slots = partial + (int64_t)bh * slots_per_head * (D + 2);
+            if (threadIdx.x < D) {
+                const int d = threadIdx.x;
+                float mw = -INFINITY;
+#pragma unroll
+                for (int w = 0; w < WARPS; ++w) mw = fmaxf(mw, s_m[w]);
+                float L = 0.f, A = 0.f;
+#pragma unroll
+                for (int w = 0; w < WARPS; ++w) {
+                    const float cw = s_m[w] > -INFINITY ? expf(s_m[w] - mw) : 0.f;
+                    L += s_l[w] * cw;
+                    A += s_acc[w][d] * cw;
+                }
+                if (whole) {
+                    out[(int64_t)bh * D + d] = from_f<T>(A / L * v_scale[bh % H]);  // FP8: V's scale, once
+                } else {
+                    float *pp = slots + (int64_t)((int)blockIdx.x - first_cta) * (D + 2);
+                    __stcg(pp + 2 + d, A);
+                    if (d == 0) {
+                        __stcg(pp, mw);
+                        __stcg(pp + 1, L);
+                    }
+                    __threadfence();
+                }
+            }
+            if (!whole) {
+                named_bar_sync(1, CONSUMERS);
+                if (threadIdx.x == 0) {
+                    const int old = atomicAdd(tickets + bh, 1);
+                    s_last = old == nseg - 1;
+                    if (s_last) tickets[bh] = 0;  // self-cleaning: every other sharer has already arrived
+                    __threadfence();
+                }
+                named_bar_sync(1, CONSUMERS);
+                if (s_last && threadIdx.x < D) {
+                    const int d = threadIdx.x;
+                    float mw = -INFINITY;
+                    for (int s = 0; s < nseg; ++s) mw = fmaxf(mw, __ldcg(slots + (int64_t)s * (D + 2)));
+                    float L = 0.f, A = 0.f;
+                    for (int s = 0; s < nseg; ++s) {
+                        const float *pp = slots + (int64_t)s * (D + 2);
+                        const float ms = __ldcg(pp);
+                        const float cw = ms > -INFINITY ? expf(ms - mw) : 0.f;
+                        L += __ldcg(pp + 1) * cw;
+                        A += __ldcg(pp + 2 + d) * cw;
+                    }
+                    out[(int64_t)bh * D + d] = from_f<T>(A / L * v_scale[bh % H]);
+                }
+            }
+            named_bar_sync(1, CONSUMERS);  // s_acc / s_m / s_last are reused by the next segment
+        }
+        next_unit();
+    }
+}
+
+// ------------------------------------------------------------------------------------------------------------------
+// attn_gqa_kv8_kernel: attn_gqa_kernel over an FP8 E4M3 cache (uint8_t codes, one fp32 scale per KV head).  Same dealing,
+// ring, tickets, merge and workspace; a chunk keeps 16 KiB per copy, so it holds twice the rows (128 / 256 at D = 128 / 64).
+// The mma.sync B fragments are built from code pairs widened by e4m3x2_to (K: one 16-byte load per row and 64 columns; V:
+// one 1- or 2-byte load per row); the appended row is quantised in registers and enters the ring as codes.
+// ------------------------------------------------------------------------------------------------------------------
+template <typename T, int D, int QT, bool ROPE>
+__device__ __forceinline__ void
+    attn_gqa_kv8_body(uint8_t *__restrict__ kcache, uint8_t *__restrict__ vcache, const T *__restrict__ q,
+                    const T *__restrict__ kin, const T *__restrict__ vin, const void *__restrict__ position_id,
+                    int pos_flags, T *__restrict__ out, int Smax, int Bn, int Hkv, int G, int NQG,
+                    float *__restrict__ partial, int slots_per_head, int *__restrict__ tickets, const void *__restrict__ rope_pos, int rope_pos_dtype,
+                    const float *__restrict__ k_scale, const float *__restrict__ v_scale) {
+    using KT = uint8_t;
+    using C = RowCfg<T, D>;
+    using Q = GqaCfg<T, D, KT>;
+    constexpr int EPL = C::EPL, LPR = C::LPR, RPW = C::RPW;
+    constexpr int CH = Q::CH, NC = Q::NC, NT = Q::NT, NJ = Q::NJ, QLD = Q::QLD, PLD = Q::PLD;
+    constexpr int GP = 16 * QT;  // padded query rows
+    constexpr int CHUNK_BYTES = CH * D * (int)sizeof(KT);
+    constexpr int CONSUMERS = GQ_WARPS * 32;
+    constexpr bool MMA = sizeof(T) == 2;
+    constexpr float kScale = attn_scale<D>();
+    extern __shared__ __align__(128) unsigned char ring[];  // stages x { K chunk | V chunk }
+    __shared__ __align__(8) uint64_t full[AS_STAGES], empty[AS_STAGES];
+    __shared__ __align__(16) T s_q[GP * QLD];   // (rotated) query rows of the current query group
+    __shared__ __align__(16) T s_p[GP * PLD];   // P of the current chunk, rounded to T
+    __shared__ __align__(16) T s_plo[MMA ? GP * PLD : 1];  // f16 / bf16: P - s_p, rounded to T
+    __shared__ float s_red[2][GQ_WARPS][GP];    // per-warp row maxima / row sums of the current chunk
+    __shared__ float s_cs[D / 2], s_sn[D / 2];
+    __shared__ int s_last;
+    __shared__ int s_pre[AS_MAX_B + 1];  // (KV head, query group, chunk) units before batch row b; s_pre[B] = total
+
+    pdl_trigger();
+    const int pos_dtype = pos_flags & 0xff;
+    const bool per_row = (pos_flags & ITB_POS_PER_ROW) != 0;
+    if (pos_flags & ITB_POS_IN_STEP) pdl_wait();  // (see attn_stream_kernel)
+    auto pos_of = [&](int b) {
+        const int p = pos_dtype == ITB_I64 ? read_pos<int64_t>(position_id, per_row ? b : 0)
+                                           : read_pos<int32_t>(position_id, per_row ? b : 0);
+        return min(max(p, 0), Smax - 1);
+    };
+    if (threadIdx.x == 0) {
+        for (int s = 0; s < AS_STAGES; ++s) {
+            mbar_init(&full[s], 1);
+            mbar_init(&empty[s], GQ_WARPS);
+        }
+        fence_mbar_init();
+    }
+    // V rows past a chunk's valid rows enter the P.V product with P = 0: they must hold finite values, so the ring starts
+    // zeroed (later it only ever holds cache rows)
+    for (int i = threadIdx.x; i < AS_STAGES * 2 * CHUNK_BYTES / 16; i += blockDim.x)
+        reinterpret_cast<uint4 *>(ring)[i] = make_uint4(0, 0, 0, 0);
+    fence_proxy_async();
+    const int HV = Hkv * NQG;  // (KV head, query group) segments per batch row
+    for (int b = threadIdx.x; b < Bn; b += blockDim.x) s_pre[b] = HV * (pos_of(b) / CH + 1);
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        int acc = 0;
+        for (int b = 0; b < Bn; ++b) {
+            const int n = s_pre[b];
+            s_pre[b] = acc;
+            acc += n;
+        }
+        s_pre[Bn] = acc;
+    }
+    __syncthreads();
+
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int BH = Bn * HV;
+    const int64_t total = s_pre[Bn], ncta = min((int64_t)gridDim.x, total);
+    if (blockIdx.x >= ncta) return;
+    int nunits, bh, c, brow, pos, nch;  // bh = (b * Hkv + KV head) * NQG + query group
+    {
+        const int64_t u0 = blockIdx.x * total / ncta, u1 = (blockIdx.x + 1) * total / ncta;
+        nunits = (int)(u1 - u0);
+        brow = 0;
+        while (brow + 1 < Bn && s_pre[brow + 1] <= u0) ++brow;
+        pos = pos_of(brow);
+        nch = pos / CH + 1;
+        const int r = (int)(u0 - s_pre[brow]);
+        bh = brow * HV + r / nch;
+        c = r % nch;
+    }
+    auto next_unit = [&]() {
+        if (++c == nch) {
+            c = 0;
+            ++bh;
+            if (bh % HV == 0 && bh < BH) {
+                brow = bh / HV;
+                pos = pos_of(brow);
+                nch = pos / CH + 1;
+            }
+        }
+    };
+
+    if (warp == GQ_WARPS) {
+        // ---------------- producer (as attn_stream_kernel) ----------------
+        if (lane == 0) {
+            const uint64_t policy = l2_policy_evict_first();
+            int st = 0, ph = 0;
+            for (int it = 0; it < nunits; ++it) {
+                mbar_wait(&empty[st], ph ^ 1);
+                const int rows = min(CH, pos - c * CH);
+                if (rows > 0) {
+                    const uint32_t bytes = (uint32_t)rows * D * (uint32_t)sizeof(KT);
+                    const int64_t off = ((int64_t)(bh / NQG) * Smax + (int64_t)c * CH) * D;
+                    mbar_expect_tx(&full[st], 2 * bytes);
+                    bulk_load_1d(ring + (size_t)st * 2 * CHUNK_BYTES, kcache + off, bytes, &full[st], policy);
+                    bulk_load_1d(ring + (size_t)st * 2 * CHUNK_BYTES + CHUNK_BYTES, vcache + off, bytes, &full[st], policy);
+                } else {
+                    mbar_arrive(&full[st]);
+                }
+                next_unit();
+                if (++st == AS_STAGES) { st = 0; ph ^= 1; }
+            }
+        }
+        return;
+    }
+
+    // ---------------- consumers ----------------
+    int table_b = -1;
+    auto rope_table = [&](int b) {
+        if (threadIdx.x < D / 2) {
+            const float p = rope_pos_dtype == ITB_I64 ? (float)(int)((const int64_t *)rope_pos)[b]
+                                                      : (float)((const int32_t *)rope_pos)[b];
+            const float freq = p * powf(10000.f, -(float)(threadIdx.x * 2) / (float)D);
+            s_cs[threadIdx.x] = round_t<T>(cosf(freq));
+            s_sn[threadIdx.x] = round_t<T>(sinf(freq));
+        }
+        named_bar_sync(1, CONSUMERS);
+        table_b = b;
+    };
+    if (ROPE) rope_table(bh / HV);
+    pdl_wait();
+    const int sub = lane / LPR, col = (lane % LPR) * EPL;  // row-load layout (q, appended k / v)
+    const int qr = lane >> 2, qc = lane & 3;               // fragment layout: rows qr, qr + 8 of each 16-row tile
+    const int cw = warp * (CH / GQ_WARPS);                 // first chunk row of this warp's S columns
+    // o[t][j][2h + e]: row 16t + qr + 8h, column 8 NJ w + 8j + 2qc + e
+    float m_run[QT][2], l_run[QT][2], o[QT][NJ][4];
+    bool seg_from_start = false;
+    int st = 0, ph = 0;
+    int64_t q0 = 0;  // first query head of the segment's group
+    int gq = 0;      // query heads in the segment's group (<= GP)
+    for (int it = 0; it < nunits; ++it) {
+        if (it == 0 || c == 0) {
+            // new segment: reset the running softmax, stage the group's query rows (rotated if asked)
+            seg_from_start = c == 0;
+#pragma unroll
+            for (int t = 0; t < QT; ++t)
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                    m_run[t][h] = -INFINITY;
+                    l_run[t][h] = 0.f;
+#pragma unroll
+                    for (int j = 0; j < NJ; ++j) o[t][j][2 * h] = o[t][j][2 * h + 1] = 0.f;
+                }
+            if (ROPE && bh / HV != table_b) rope_table(bh / HV);
+            // query heads [kvh G + qg GP, + gq) of batch row b
+            q0 = (int64_t)(bh / NQG) * G + (int64_t)(bh % NQG) * GP;
+            gq = min(GP, G - (bh % NQG) * GP);
+            const T *qh = q + q0 * D;
+            for (int r0 = warp * RPW; r0 < GP; r0 += GQ_WARPS * RPW) {
+                const int r = r0 + sub;
+                Vec16<T> x;
+                *reinterpret_cast<uint4 *>(x.v) = make_uint4(0, 0, 0, 0);
+                if (r < gq) x = ld16(qh + (int64_t)r * D + col);
+                if (ROPE) rope_one<T, D, EPL, LPR>(x, col, s_cs, s_sn);
+                st16(s_q + r * QLD + col, x);
+            }
+            named_bar_sync(1, CONSUMERS);
+        }
+        const int nvalid = pos - c * CH;  // cache rows of this chunk below the position (last chunk: < CH)
+        const bool last_chunk = c == nch - 1;
+        KT *ks = reinterpret_cast<KT *>(ring + (size_t)st * 2 * CHUNK_BYTES), *vs = ks + CH * D;
+        mbar_wait(&full[st], ph);
+        int nrows = min(nvalid, CH);
+        if (last_chunk) {
+            // the row appended this step: rotate k if asked, store k / v into ring row nvalid, and (group 0) in place
+            if (warp == 0) {
+                const int64_t kv = bh / NQG;
+#pragma unroll
+                for (int r0 = 0; r0 < 2; r0 += RPW) {
+                    const int which = r0 + sub;  // 0: k, 1: v
+                    Vec16<T> x = ld16((which == 0 ? kin : vin) + kv * D + col);
+                    if (ROPE) {
+                        Vec16<T> xr = x;
+                        rope_one<T, D, EPL, LPR>(xr, col, s_cs, s_sn);
+                        if (which == 0) x = xr;
+                    }
+                    if (RPW <= 2 || which < 2) {  // (D = 64, 2-byte types: sub-rows 2, 3 only took part in the shuffles)
+                        // quantised in registers; the ring row holds the codes, so the row contributes through them
+                        const uint2 codes = quantise_e4m3x8(x, (which == 0 ? k_scale : v_scale)[kv % Hkv]);
+                        if (bh % NQG == 0)
+                            *reinterpret_cast<uint2 *>((which == 0 ? kcache : vcache) + (kv * Smax + pos) * D + col) = codes;
+                        *reinterpret_cast<uint2 *>((which == 0 ? ks : vs) + nvalid * D + col) = codes;
+                    }
+                }
+                fence_proxy_async();  // the producer's next bulk copy into this stage must land after these stores
+            }
+            named_bar_sync(1, CONSUMERS);
+            nrows = nvalid + 1;
+        }
+
+        // ---- S = Q K^T for this warp's chunk rows, scaled, masked past nrows: s[t][h][e] = S[16t + qr + 8h][cw + NC qc + e]
+        float s[QT][2][NC];
+        // The k (head-dim) order inside each 64-column block is permuted, alike for Q and K, so that a thread's B fragments
+        // come from one 16-byte load of codes: k16 step 4jj + st, fragment column pair 2qc + {0,1} (+8) <-> columns
+        // 64jj + 16qc + 4st + {0,1} ({2,3}).  n8 tile j, B column n = chunk row cw + NC (n >> 1) + 2j + (n & 1): the
+        // thread's accumulator columns 2qc, 2qc + 1 of every tile land on its NC consecutive chunk rows.
+        constexpr int KS = D / 16;
+        const float ksc = k_scale[(bh / NQG) % Hkv] * kScale;  // the KV head's K scale with 1/sqrt(D)
+        uint32_t kf[NT][KS][2];
+        const int krow = cw + NC * (qr >> 1) + (qr & 1);
+#pragma unroll
+        for (int j = 0; j < NT; ++j)
+#pragma unroll
+            for (int jj = 0; jj < D / 64; ++jj) {
+                const uint4 raw = *reinterpret_cast<const uint4 *>(ks + (krow + 2 * j) * D + 64 * jj + 16 * qc);
+                const uint32_t w[4] = {raw.x, raw.y, raw.z, raw.w};
+#pragma unroll
+                for (int st4 = 0; st4 < 4; ++st4) {
+                    kf[j][4 * jj + st4][0] = e4m3x2_to<T>(w[st4]);
+                    kf[j][4 * jj + st4][1] = e4m3x2_to<T>(w[st4] >> 16);
+                }
+            }
+#pragma unroll
+        for (int t = 0; t < QT; ++t) {
+            float acc[NT][4];
+#pragma unroll
+            for (int j = 0; j < NT; ++j) acc[j][0] = acc[j][1] = acc[j][2] = acc[j][3] = 0.f;
+#pragma unroll
+            for (int jj = 0; jj < D / 64; ++jj) {
+                const T *qa = s_q + (16 * t + qr) * QLD + 64 * jj + 16 * qc;
+                const uint4 x0 = *reinterpret_cast<const uint4 *>(qa), x1 = *reinterpret_cast<const uint4 *>(qa + 8);
+                const uint4 y0 = *reinterpret_cast<const uint4 *>(qa + 8 * QLD), y1 = *reinterpret_cast<const uint4 *>(qa + 8 * QLD + 8);
+                const uint32_t wa[8] = {x0.x, x0.y, x0.z, x0.w, x1.x, x1.y, x1.z, x1.w};
+                const uint32_t wb[8] = {y0.x, y0.y, y0.z, y0.w, y1.x, y1.y, y1.z, y1.w};
+#pragma unroll
+                for (int st4 = 0; st4 < 4; ++st4) {
+                    uint32_t a[4] = {wa[2 * st4], wb[2 * st4], wa[2 * st4 + 1], wb[2 * st4 + 1]};
+#pragma unroll
+                    for (int j = 0; j < NT; ++j) mma_m16n8k16<T>(acc[j], a, kf[j][4 * jj + st4][0], kf[j][4 * jj + st4][1]);
+                }
+            }
+#pragma unroll
+            for (int j = 0; j < NT; ++j)
+#pragma unroll
+                for (int h = 0; h < 2; ++h)
+#pragma unroll
+                    for (int e = 0; e < 2; ++e) s[t][h][2 * j + e] = acc[j][2 * h + e] * ksc;
+        }
+        // ---- softmax: chunk row maxima across the warps, then P and its row sums
+#pragma unroll
+        for (int t = 0; t < QT; ++t)
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                float mx = -INFINITY;
+#pragma unroll
+                for (int e = 0; e < NC; ++e) {
+                    if (cw + NC * qc + e >= nrows) s[t][h][e] = -INFINITY;
+                    mx = fmaxf(mx, s[t][h][e]);
+                }
+                mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+                mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+                if (qc == 0) s_red[0][warp][16 * t + qr + 8 * h] = mx;
+            }
+        named_bar_sync(1, CONSUMERS);
+        float corr[QT][2];
+#pragma unroll
+        for (int t = 0; t < QT; ++t)
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                const int r = 16 * t + qr + 8 * h;
+                float cm = -INFINITY;
+#pragma unroll
+                for (int w = 0; w < GQ_WARPS; ++w) cm = fmaxf(cm, s_red[0][w][r]);
+                const float mnew = fmaxf(m_run[t][h], cm);  // finite: every chunk has >= 1 row
+                float sum = 0.f;
+                __align__(NC * sizeof(T)) T hi[NC], lo[NC];
+#pragma unroll
+                for (int e = 0; e < NC; ++e) {
+                    const float p = expf(s[t][h][e] - mnew);  // masked: exp(-inf) = 0
+                    hi[e] = from_f<T>(p);
+                    lo[e] = from_f<T>(p - to_f(hi[e]));
+                    sum += p;
+                }
+                if constexpr (MMA) {
+                    using PW = std::conditional_t<NC == 2, uint32_t, std::conditional_t<NC == 4, uint2, uint4>>;  // the thread's NC weights in one store
+                    *reinterpret_cast<PW *>(s_p + r * PLD + cw + NC * qc) = *reinterpret_cast<const PW *>(hi);
+                    *reinterpret_cast<PW *>(s_plo + r * PLD + cw + NC * qc) = *reinterpret_cast<const PW *>(lo);
+                } else {
+#pragma unroll
+                    for (int e = 0; e < NC; ++e) s_p[r * PLD + cw + NC * qc + e] = hi[e];
+                }
+                sum += __shfl_xor_sync(0xffffffffu, sum, 1);
+                sum += __shfl_xor_sync(0xffffffffu, sum, 2);
+                if (qc == 0) s_red[1][warp][r] = sum;
+                corr[t][h] = expf(m_run[t][h] - mnew);  // m_run = -inf -> 0
+                m_run[t][h] = mnew;
+            }
+        named_bar_sync(1, CONSUMERS);
+#pragma unroll
+        for (int t = 0; t < QT; ++t)
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                float ls = 0.f;
+#pragma unroll
+                for (int w = 0; w < GQ_WARPS; ++w) ls += s_red[1][w][16 * t + qr + 8 * h];
+                l_run[t][h] = l_run[t][h] * corr[t][h] + ls;
+#pragma unroll
+                for (int j = 0; j < NJ; ++j) {
+                    o[t][j][2 * h] *= corr[t][h];
+                    o[t][j][2 * h + 1] *= corr[t][h];
+                }
+            }
+        // ---- O += P V over output columns [8 NJ w, 8 NJ (w + 1))
+        // B fragment of k16 step kk, tile j: V codes of chunk rows 16kk + 2qc + {0, 1} (b0) and + {8, 9} (b1) in column
+        // 8 NJ w + NJ qr + j (ocol): one NJ-byte load per row serves every tile
+        const KT *vcol = vs + 8 * NJ * warp + NJ * qr;
+#pragma unroll 4
+        for (int kk = 0; kk < CH / 16; ++kk) {
+            const KT *r0 = vcol + (16 * kk + 2 * qc) * D;
+            uint32_t x[4];
+#pragma unroll
+            for (int i = 0; i < 4; ++i) {
+                const KT *ri = r0 + ((i & 1) + 8 * (i >> 1)) * D;  // rows +0, +1, +8, +9
+                if constexpr (NJ == 2) x[i] = *reinterpret_cast<const uint16_t *>(ri);
+                else x[i] = *ri;
+            }
+#pragma unroll
+            for (int j = 0; j < NJ; ++j) {
+                const uint32_t sel = j == 0 ? 0x0040u : 0x0051u;  // byte j of the two rows -> a code pair
+                const uint32_t b0 = e4m3x2_to<T>(__byte_perm(x[0], x[1], sel));
+                const uint32_t b1 = e4m3x2_to<T>(__byte_perm(x[2], x[3], sel));
+#pragma unroll
+                for (int t = 0; t < QT; ++t) {
+                    const int off = (16 * t + (lane & 15)) * PLD + 16 * kk + 8 * (lane >> 4);
+                    uint32_t a[4];
+                    ldmatrix_x4(a[0], a[1], a[2], a[3], smem_u32(s_plo + off));
+                    mma_m16n8k16<T>(o[t][j], a, b0, b1);
+                    ldmatrix_x4(a[0], a[1], a[2], a[3], smem_u32(s_p + off));
+                    mma_m16n8k16<T>(o[t][j], a, b0, b1);
+                }
+            }
+        }
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&empty[st]);
+        if (++st == AS_STAGES) { st = 0; ph ^= 1; }
+
+        if (last_chunk || it == nunits - 1) {
+            // ---- segment end: write O / l, or this CTA's partial; the last CTA of a shared segment merges its gq rows
+            const bool whole = seg_from_start && last_chunk;
+            const int64_t hu0 = (int64_t)s_pre[brow] + (int64_t)(bh - brow * HV) * nch;  // first unit of this segment
+            const int first_cta = (int)(((hu0 + 1) * ncta - 1) / total);
+            const int last_cta = (int)(((hu0 + nch) * ncta - 1) / total);
+            const int nseg = last_cta - first_cta + 1;
+#pragma unroll
+            for (int t = 0; t < QT; ++t)
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                    const int r = 16 * t + qr + 8 * h;
+                    if (r >= gq) continue;
+                    // the n8 tiles' columns interleave (see O += P V): tile j, element e is column 8 NJ w + NJ (2qc + e) + j
+                    const float vsc = v_scale[(bh / NQG) % Hkv];
+                    const int c0 = 8 * NJ * warp + 2 * NJ * qc;
+                    float *pp = whole ? nullptr : partial + ((q0 + r) * slots_per_head + ((int)blockIdx.x - first_cta)) * (D + 2) + 2;
+#pragma unroll
+                    for (int j = 0; j < NJ; ++j)
+#pragma unroll
+                        for (int e = 0; e < 2; ++e) {
+                            if (whole) out[(q0 + r) * D + c0 + NJ * e + j] = from_f<T>(o[t][j][2 * h + e] / l_run[t][h] * vsc);
+                            else __stcg(pp + c0 + NJ * e + j, o[t][j][2 * h + e]);
+                        }
+                    if (!whole && warp == 0 && qc == 0) {
+                        __stcg(pp - 2, m_run[t][h]);
+                        __stcg(pp - 1, l_run[t][h]);
+                    }
+                }
+            if (!whole) {
+                __threadfence();
+                named_bar_sync(1, CONSUMERS);
+                if (threadIdx.x == 0) {
+                    const int old = atomicAdd(tickets + bh, 1);
+                    s_last = old == nseg - 1;
+                    if (s_last) tickets[bh] = 0;  // self-cleaning: every other sharer has already arrived
+                    __threadfence();
+                }
+                named_bar_sync(1, CONSUMERS);
+                if (s_last) {
+                    for (int i = threadIdx.x; i < gq * D; i += CONSUMERS) {
+                        const int r = i / D, d = i % D;
+                        const float *slots = partial + (q0 + r) * slots_per_head * (D + 2);
+                        float mw = -INFINITY;
+                        for (int s2 = 0; s2 < nseg; ++s2) mw = fmaxf(mw, __ldcg(slots + (int64_t)s2 * (D + 2)));
+                        float L = 0.f, A = 0.f;
+                        for (int s2 = 0; s2 < nseg; ++s2) {
+                            const float *pp = slots + (int64_t)s2 * (D + 2);
+                            const float cw2 = expf(__ldcg(pp) - mw);  // every partial holds >= 1 row: finite m
+                            L += __ldcg(pp + 1) * cw2;
+                            A += __ldcg(pp + 2 + d) * cw2;
+                        }
+                        out[(q0 + r) * D + d] = from_f<T>(A / L * v_scale[(bh / NQG) % Hkv]);
+                    }
+                }
+            }
+            named_bar_sync(1, CONSUMERS);  // s_q / s_last are reused by the next segment
+        }
+        next_unit();
+    }
+}
+
 // The kernels: one name per head width, so that the 128-wide kernels keep the names profiles and tests know them by
 #define ITB_ATTN_STREAM_ARGS                                                                                            \
     T *__restrict__ kcache, T *__restrict__ vcache, const T *__restrict__ q, const T *__restrict__ kin,              \
@@ -920,6 +1724,25 @@ __global__ void __launch_bounds__((GQ_WARPS + 1) * 32, AS_CTAS_PER_SM) attn_gqa6
     attn_gqa_body<T, 64, QT, ROPE>(ITB_ATTN_GQA_PASS);  // (pdl_trigger / pdl_wait inside)
 }
 
+// FP8 E4M3 caches: uint8_t codes + one fp32 scale per KV head, f16 / bf16 activations, both widths in one name each
+#define ITB_ATTN_KV8_ARGS(...)                                                                                          \
+    uint8_t *__restrict__ kcache, uint8_t *__restrict__ vcache, const T *__restrict__ q, const T *__restrict__ kin,  \
+        const T *__restrict__ vin, const void *__restrict__ position_id, int pos_flags, T *__restrict__ out, int Smax, \
+        __VA_ARGS__, const void *__restrict__ rope_pos, int rope_pos_dtype
+template <typename T, int D, int WARPS, int U, bool ROPE>
+__global__ void __launch_bounds__((WARPS + 1) * 32, AS_CTAS_PER_SM)
+    attn_stream_kv8_kernel(ITB_ATTN_KV8_ARGS(int BH, float *__restrict__ partial, int slots_per_head, int *__restrict__ tickets),
+                           int H, const float *__restrict__ k_scale, const float *__restrict__ v_scale) {
+    attn_stream_kv8_body<T, D, WARPS, U, ROPE>(ITB_ATTN_STREAM_PASS, k_scale, v_scale);  // (pdl_trigger / pdl_wait inside)
+}
+template <typename T, int D, int QT, bool ROPE>
+__global__ void __launch_bounds__((GQ_WARPS + 1) * 32, AS_CTAS_PER_SM)
+    attn_gqa_kv8_kernel(ITB_ATTN_KV8_ARGS(int Bn, int Hkv, int G, int NQG, float *__restrict__ partial, int slots_per_head,
+                                          int *__restrict__ tickets),
+                        const float *__restrict__ k_scale, const float *__restrict__ v_scale) {
+    attn_gqa_kv8_body<T, D, QT, ROPE>(ITB_ATTN_GQA_PASS, k_scale, v_scale);  // (pdl_trigger / pdl_wait inside)
+}
+
 }  // namespace itb
 
 using namespace itb;
@@ -930,79 +1753,89 @@ extern "C" int64_t it_b200_attention_kvcache_workspace(int B, int H, int S_max, 
     return (int64_t)B * H * stream_slots_per_head(S_max) * (D + 2) * sizeof(float);
 }
 
-template <typename T, int D, bool ROPE>
-static int launch_attn_stream(T *kc, T *vc, const T *q, const T *k, const T *v, const void *position_id, int pos_flags,
+template <typename T, typename KT, int D, bool ROPE>
+static int launch_attn_stream(KT *kc, KT *vc, const T *q, const T *k, const T *v, const void *position_id, int pos_flags,
                               const void *rope_pos, int rope_pos_dtype, T *out, int BH, int H, int S_max,
-                              float *workspace, cudaStream_t st) {
+                              float *workspace, const float *k_scale, const float *v_scale, cudaStream_t st) {
     constexpr int WARPS = 8, U = 4;  // consumer warps x rows per lane and chunk
-    constexpr int CH = WARPS * RowCfg<T, D>::RPW * U;
-    const size_t smem = (size_t)AS_STAGES * 2 * CH * D * sizeof(T);
-    auto kern = D == 128 ? attn_stream_kernel<T, WARPS, U, ROPE> : attn_stream64_kernel<T, WARPS, U, ROPE>;
-    // the attribute is per DEVICE: a process may own runtimes on several GPUs
-    if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) return 1;
+    constexpr int CH = WARPS * RowCfg<KT, D>::RPW * U;
+    const size_t smem = (size_t)AS_STAGES * 2 * CH * D * sizeof(KT);
     int *tickets = stream_tickets(st, BH);
     if (!tickets) return 1;
     const int64_t max_units = (int64_t)BH * (S_max / CH + 1);
     const int grid = (int)std::min<int64_t>(max_units, (int64_t)AS_CTAS_PER_SM * kNumSMs);
-    cudaError_t e = launch_k(kern, dim3(grid), dim3((WARPS + 1) * 32), smem, st, kc, vc, q, k, v, position_id, pos_flags,
-                             out, S_max, BH, workspace, stream_slots_per_head(S_max), tickets, rope_pos, rope_pos_dtype, H);
+    cudaError_t e;
+    if constexpr (std::is_same_v<KT, uint8_t>) {
+        auto kern = attn_stream_kv8_kernel<T, D, WARPS, U, ROPE>;
+        if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) return 1;
+        e = launch_k(kern, dim3(grid), dim3((WARPS + 1) * 32), smem, st, kc, vc, q, k, v, position_id, pos_flags, out, S_max,
+                     BH, workspace, stream_slots_per_head(S_max), tickets, rope_pos, rope_pos_dtype, H, k_scale, v_scale);
+    } else {
+        auto kern = D == 128 ? attn_stream_kernel<T, WARPS, U, ROPE> : attn_stream64_kernel<T, WARPS, U, ROPE>;
+        // the attribute is per DEVICE: a process may own runtimes on several GPUs
+        if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) return 1;
+        e = launch_k(kern, dim3(grid), dim3((WARPS + 1) * 32), smem, st, kc, vc, q, k, v, position_id, pos_flags, out, S_max,
+                     BH, workspace, stream_slots_per_head(S_max), tickets, rope_pos, rope_pos_dtype, H);
+    }
     return e == cudaSuccess ? 0 : 1;
 }
 
-template <typename T, int D, int QT, bool ROPE>
-static int launch_attn_gqa(T *kc, T *vc, const T *q, const T *k, const T *v, const void *position_id, int pos_flags,
+template <typename T, typename KT, int D, int QT, bool ROPE>
+static int launch_attn_gqa(KT *kc, KT *vc, const T *q, const T *k, const T *v, const void *position_id, int pos_flags,
                            const void *rope_pos, int rope_pos_dtype, T *out, int B, int Hkv, int G, int S_max,
-                           float *workspace, cudaStream_t st) {
-    constexpr int CH = GqaCfg<T, D>::CH;
-    const size_t smem = (size_t)AS_STAGES * 2 * CH * D * sizeof(T);
-    auto kern = D == 128 ? attn_gqa_kernel<T, QT, ROPE> : attn_gqa64_kernel<T, QT, ROPE>;
-    if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) return 1;
+                           float *workspace, const float *k_scale, const float *v_scale, cudaStream_t st) {
+    constexpr int CH = GqaCfg<T, D, KT>::CH;
+    const size_t smem = (size_t)AS_STAGES * 2 * CH * D * sizeof(KT);
     const int nqg = (G + 16 * QT - 1) / (16 * QT);  // query groups per KV head
     int *tickets = stream_tickets(st, B * Hkv * nqg);
     if (!tickets) return 1;
     const int64_t max_units = (int64_t)B * Hkv * nqg * (S_max / CH + 1);
     const int grid = (int)std::min<int64_t>(max_units, (int64_t)AS_CTAS_PER_SM * kNumSMs);
-    cudaError_t e = launch_k(kern, dim3(grid), dim3((GQ_WARPS + 1) * 32), smem, st, kc, vc, q, k, v, position_id, pos_flags,
-                             out, S_max, B, Hkv, G, nqg, workspace, stream_slots_per_head(S_max), tickets, rope_pos,
-                             rope_pos_dtype);
+    cudaError_t e;
+    if constexpr (std::is_same_v<KT, uint8_t>) {
+        auto kern = attn_gqa_kv8_kernel<T, D, QT, ROPE>;
+        if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) return 1;
+        e = launch_k(kern, dim3(grid), dim3((GQ_WARPS + 1) * 32), smem, st, kc, vc, q, k, v, position_id, pos_flags, out, S_max,
+                     B, Hkv, G, nqg, workspace, stream_slots_per_head(S_max), tickets, rope_pos, rope_pos_dtype, k_scale,
+                     v_scale);
+    } else {
+        auto kern = D == 128 ? attn_gqa_kernel<T, QT, ROPE> : attn_gqa64_kernel<T, QT, ROPE>;
+        if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) return 1;
+        e = launch_k(kern, dim3(grid), dim3((GQ_WARPS + 1) * 32), smem, st, kc, vc, q, k, v, position_id, pos_flags, out, S_max,
+                     B, Hkv, G, nqg, workspace, stream_slots_per_head(S_max), tickets, rope_pos, rope_pos_dtype);
+    }
     return e == cudaSuccess ? 0 : 1;
 }
 
-// one query tile of 16 rows for G <= 16, else groups of two tiles (four tiles spill registers and, for fp32, exceed the
-// static shared memory)
-template <typename T, int D, bool ROPE>
-static int launch_attn_gqa_tiles(T *kc, T *vc, const T *q, const T *k, const T *v, const void *position_id, int pos_flags,
-                                 const void *rope_pos, int rope_pos_dtype, T *out, int B, int Hkv, int G, int S_max,
-                                 float *workspace, cudaStream_t st) {
-    if (G <= 16)
-        return launch_attn_gqa<T, D, 1, ROPE>(kc, vc, q, k, v, position_id, pos_flags, rope_pos, rope_pos_dtype, out, B, Hkv, G,
-                                              S_max, workspace, st);
-    return launch_attn_gqa<T, D, 2, ROPE>(kc, vc, q, k, v, position_id, pos_flags, rope_pos, rope_pos_dtype, out, B, Hkv, G,
-                                          S_max, workspace, st);
-}
-
-// the kernel for head width D, with RoPE folded in when rope_pos is given
-template <typename T, int D>
-static int launch_attn_width(T *kc, T *vc, const T *q, const T *k, const T *v, const void *position_id, int pos_flags,
+// the kernel for head width D and G = Hq / Hkv, with RoPE folded in when rope_pos is given.  G > 1 takes one query tile of
+// 16 rows for G <= 16, else groups of two tiles (four tiles spill registers and, for fp32, exceed the static shared memory)
+template <typename T, typename KT, int D>
+static int launch_attn_width(KT *kc, KT *vc, const T *q, const T *k, const T *v, const void *position_id, int pos_flags,
                              const void *rope_pos, int rope_pos_dtype, T *out, int B, int Hq, int Hkv, int S_max,
-                             float *workspace, cudaStream_t st) {
+                             float *workspace, const float *k_scale, const float *v_scale, cudaStream_t st) {
     const int G = Hq / Hkv;
-    if (G > 1)
-        return rope_pos ? launch_attn_gqa_tiles<T, D, true>(kc, vc, q, k, v, position_id, pos_flags, rope_pos, rope_pos_dtype,
-                                                            out, B, Hkv, G, S_max, workspace, st)
-                        : launch_attn_gqa_tiles<T, D, false>(kc, vc, q, k, v, position_id, pos_flags, nullptr, 0, out, B,
-                                                             Hkv, G, S_max, workspace, st);
-    return rope_pos ? launch_attn_stream<T, D, true>(kc, vc, q, k, v, position_id, pos_flags, rope_pos, rope_pos_dtype, out,
-                                                     B * Hq, Hq, S_max, workspace, st)
-                    : launch_attn_stream<T, D, false>(kc, vc, q, k, v, position_id, pos_flags, nullptr, 0, out, B * Hq, Hq,
-                                                      S_max, workspace, st);
+    auto go = [&](auto rope) {
+        constexpr bool R = decltype(rope)::value;
+        const void *rp = R ? rope_pos : nullptr;
+        const int rpd = R ? rope_pos_dtype : 0;
+        if (G == 1)
+            return launch_attn_stream<T, KT, D, R>(kc, vc, q, k, v, position_id, pos_flags, rp, rpd, out, B * Hq, Hq, S_max,
+                                                   workspace, k_scale, v_scale, st);
+        if (G <= 16)
+            return launch_attn_gqa<T, KT, D, 1, R>(kc, vc, q, k, v, position_id, pos_flags, rp, rpd, out, B, Hkv, G, S_max,
+                                                   workspace, k_scale, v_scale, st);
+        return launch_attn_gqa<T, KT, D, 2, R>(kc, vc, q, k, v, position_id, pos_flags, rp, rpd, out, B, Hkv, G, S_max,
+                                               workspace, k_scale, v_scale, st);
+    };
+    return rope_pos ? go(std::true_type{}) : go(std::false_type{});
 }
 
 // Hq query heads over Hkv cache heads.  Hq == Hkv runs attn_stream_kernel; Hq = G Hkv, G > 1, runs attn_gqa_kernel.
+// k_scale non-null: the caches hold FP8 E4M3 codes (attn_*_kv8_kernel).
 static int attention_impl(int dtype, void *k_cache, void *v_cache, const void *q, const void *k, const void *v,
                           const void *position_id, int pos_flags, const void *rope_pos, int rope_pos_dtype, void *out,
                           int B, int Hq, int Hkv, int S_max, int D, void *workspace, int64_t workspace_bytes,
-                          void *stream) {
+                          void *stream, const float *k_scale = nullptr, const float *v_scale = nullptr) {
     const int H = Hq;
     const int pos_dtype = pos_flags & 0xff;
     // 128: the reference's only width (attention_kvcache.cu:154); 64: GPT-2 / TinyLlama heads (extension)
@@ -1022,10 +1855,27 @@ static int attention_impl(int dtype, void *k_cache, void *v_cache, const void *q
     ITB_CHECK(workspace && workspace_bytes >= need, "AttentionKVCache: workspace %lld < %lld bytes",
               (long long)workspace_bytes, (long long)need);
     auto st = (cudaStream_t)stream;
+    if (k_scale) {
+        ITB_CHECK(dtype == ITB_F16 || dtype == ITB_BF16, "AttentionKVCache(FP8 cache): q / k / v must be f16 or bf16 (dtype %d)", dtype);
+        ITB_CHECK(v_scale, "AttentionKVCache(FP8 cache): the V scale is missing");
+        ITB_CHECK(((reinterpret_cast<uintptr_t>(k_scale) | reinterpret_cast<uintptr_t>(v_scale)) & 3) == 0,
+                  "AttentionKVCache(FP8 cache): scales must be 4-byte aligned");
+        auto launch = [&](auto tag) {
+            using T = decltype(tag);
+            auto go = D == 64 ? launch_attn_width<T, uint8_t, 64> : launch_attn_width<T, uint8_t, 128>;
+            return go((uint8_t *)k_cache, (uint8_t *)v_cache, (const T *)q, (const T *)k, (const T *)v, position_id, pos_flags,
+                      rope_pos, rope_pos_dtype, (T *)out, B, Hq, Hkv, S_max, (float *)workspace, k_scale, v_scale, st);
+        };
+        const int rc = dtype == ITB_F16 ? launch(__half{}) : launch(__nv_bfloat16{});
+        ITB_CHECK(rc == 0, "AttentionKVCache(FP8 cache): %s kernel launch failed: %s", Hq > Hkv ? "grouped-query" : "streaming",
+                  cudaGetErrorString(cudaGetLastError()));
+        ITB_LAUNCH_CHECK("AttentionKVCache");
+        return 0;
+    }
     ITB_DISPATCH_FLOAT(dtype, "AttentionKVCache", {
-        auto go = D == 64 ? launch_attn_width<T, 64> : launch_attn_width<T, 128>;
+        auto go = D == 64 ? launch_attn_width<T, T, 64> : launch_attn_width<T, T, 128>;
         int rc = go((T *)k_cache, (T *)v_cache, (const T *)q, (const T *)k, (const T *)v, position_id, pos_flags, rope_pos,
-                    rope_pos_dtype, (T *)out, B, Hq, Hkv, S_max, (float *)workspace, st);
+                    rope_pos_dtype, (T *)out, B, Hq, Hkv, S_max, (float *)workspace, nullptr, nullptr, st);
         ITB_CHECK(rc == 0, "AttentionKVCache: %s kernel launch failed: %s", Hq > Hkv ? "grouped-query" : "streaming",
                   cudaGetErrorString(cudaGetLastError()));
         ITB_LAUNCH_CHECK("AttentionKVCache");
@@ -1056,4 +1906,13 @@ extern "C" int it_b200_attention_kvcache_rope(int dtype, void *k_cache, void *v_
     ITB_CHECK(rope_pos != nullptr, "AttentionKVCache+RoPE: rope positions missing");
     return attention_impl(dtype, k_cache, v_cache, q_pre, k_pre, v, position_id, pos_dtype, rope_pos, rope_pos_dtype, out,
                           B, H, H, S_max, D, workspace, workspace_bytes, stream);
+}
+
+extern "C" int it_b200_attention_kvcache_fp8(int dtype, void *k_cache, void *v_cache, const void *k_scale, const void *v_scale,
+                                             const void *q, const void *k, const void *v, const void *position_id, int pos_flags,
+                                             const void *rope_pos, int rope_pos_dtype, void *out, int B, int Hq, int Hkv,
+                                             int S_max, int D, void *workspace, int64_t workspace_bytes, void *stream) {
+    ITB_CHECK(k_scale && v_scale, "AttentionKVCache(FP8 cache): k_scale and v_scale are required");
+    return attention_impl(dtype, k_cache, v_cache, q, k, v, position_id, pos_flags, rope_pos, rope_pos_dtype, out, B, Hq, Hkv,
+                          S_max, D, workspace, workspace_bytes, stream, (const float *)k_scale, (const float *)v_scale);
 }

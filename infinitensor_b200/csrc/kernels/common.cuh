@@ -125,6 +125,27 @@ template <typename T> __device__ __forceinline__ void st16(T *p, const Vec16<T> 
     *reinterpret_cast<uint4 *>(p) = *reinterpret_cast<const uint4 *>(r.v);
 }
 
+// two FP8 E4M3 codes (low byte = first element) -> two values of the activation type, exactly (every E4M3 value is
+// representable in f16 and in bf16)
+template <typename T> __device__ __forceinline__ uint32_t e4m3x2_to(uint32_t pair16);
+template <> __device__ __forceinline__ uint32_t e4m3x2_to<__half>(uint32_t pair16) {
+    uint32_t r;
+    asm("cvt.rn.f16x2.e4m3x2 %0, %1;" : "=r"(r) : "h"((unsigned short)pair16));
+    return r;
+}
+template <> __device__ __forceinline__ uint32_t e4m3x2_to<__nv_bfloat16>(uint32_t pair16) {
+    const uint32_t h2 = e4m3x2_to<__half>(pair16);
+    const float2 f = __half22float2(*reinterpret_cast<const __half2 *>(&h2));
+    const __nv_bfloat162 b = __floats2bfloat162_rn(f.x, f.y);
+    return *reinterpret_cast<const uint32_t *>(&b);
+}
+// two fp32 values -> two FP8 E4M3 codes (low byte = lo): round to nearest even, saturated to +-448, NaN kept
+__device__ __forceinline__ uint32_t f32x2_to_e4m3x2(float lo, float hi) {
+    unsigned short r;
+    asm("cvt.rn.satfinite.e4m3x2.f32 %0, %1, %2;" : "=h"(r) : "f"(hi), "f"(lo));
+    return r;
+}
+
 inline bool aligned16(const void *p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
 
 // ---- reductions -----------------------------------------------------------------------------

@@ -61,21 +61,6 @@ struct SkinnyGroups {
     const float *w_scale[SK_MAX_GROUPS];  // W8: per-output-column scale of each group's weight matrix
 };
 
-// two FP8 E4M3 codes (low byte = first element) -> two values of the activation type, exactly (every E4M3 value is
-// representable in f16 and in bf16)
-template <typename T> __device__ __forceinline__ uint32_t e4m3x2_to(uint32_t pair16);
-template <> __device__ __forceinline__ uint32_t e4m3x2_to<__half>(uint32_t pair16) {
-    uint32_t r;
-    asm("cvt.rn.f16x2.e4m3x2 %0, %1;" : "=r"(r) : "h"((unsigned short)pair16));
-    return r;
-}
-template <> __device__ __forceinline__ uint32_t e4m3x2_to<__nv_bfloat16>(uint32_t pair16) {
-    const uint32_t h2 = e4m3x2_to<__half>(pair16);
-    const float2 f = __half22float2(*reinterpret_cast<const __half2 *>(&h2));
-    const __nv_bfloat162 b = __floats2bfloat162_rn(f.x, f.y);
-    return *reinterpret_cast<const uint32_t *>(&b);
-}
-
 template <typename T, int MT, int NB, bool W8>
 __global__ void __launch_bounds__(SK_THREADS) gemm_skinny_kernel(const __grid_constant__ SkinnyGroups grp,
                                                                  const __grid_constant__ CUtensorMap mapX,

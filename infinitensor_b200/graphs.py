@@ -22,7 +22,7 @@ from dataclasses import dataclass, field
 import numpy as np
 
 F32, F16, BF16, I64, I32 = 1, 10, 16, 7, 6
-FP8 = 17  # FP8 E4M3 weight codes (SURVEY 8(f-4))
+FP8 = 17  # FP8 E4M3 codes: weights (SURVEY 8(f-4)) and, with LlamaConfig.kv_fp8, the KV caches
 LINEAR = 0
 
 
@@ -76,27 +76,28 @@ class LlamaConfig:
     dtype: int = BF16
     fp8_weights: bool = False  # the seven projection matrices of every layer + the logits head as FP8 E4M3 codes + f32 column scales
     kv_heads: int | None = None  # grouped-query attention: KV heads shared by heads // kv_heads query heads each; None = heads
+    kv_fp8: bool = False  # KV caches as FP8 E4M3 codes + per-layer f32 [KV heads] k / v scales (one token per step)
 
     @property
     def n_kv(self) -> int:
         return self.heads if self.kv_heads is None else self.kv_heads
 
     @staticmethod
-    def llama3_8b(batch=16, s_max=1024, dtype=BF16):
+    def llama3_8b(batch=16, s_max=1024, dtype=BF16, layers=32, kv_fp8=False):
         """Llama-3-8B shape: 32 query heads over 8 KV heads (G = 4)."""
-        return LlamaConfig(layers=32, d_model=4096, heads=32, kv_heads=8, head_dim=128, ffn=14336, vocab=128256,
-                           s_max=s_max, batch=batch, dtype=dtype)
+        return LlamaConfig(layers=layers, d_model=4096, heads=32, kv_heads=8, head_dim=128, ffn=14336, vocab=128256,
+                           s_max=s_max, batch=batch, dtype=dtype, kv_fp8=kv_fp8)
 
     @staticmethod
-    def tiny(dtype=BF16, layers=2, batch=4):
+    def tiny(dtype=BF16, layers=2, batch=4, kv_fp8=False):
         return LlamaConfig(layers=layers, d_model=256, heads=2, head_dim=128, ffn=512, vocab=1000, s_max=64,
-                           batch=batch, dtype=dtype)
+                           batch=batch, dtype=dtype, kv_fp8=kv_fp8)
 
     @staticmethod
-    def tinyllama_1b(batch=16, s_max=1024, dtype=BF16, layers=22):
+    def tinyllama_1b(batch=16, s_max=1024, dtype=BF16, layers=22, kv_fp8=False):
         """TinyLlama-1.1B shape: 32 query heads of 64 over 4 KV heads (G = 8)."""
         return LlamaConfig(layers=layers, d_model=2048, heads=32, kv_heads=4, head_dim=64, ffn=5632, vocab=32000,
-                           s_max=s_max, batch=batch, dtype=dtype)
+                           s_max=s_max, batch=batch, dtype=dtype, kv_fp8=kv_fp8)
 
     def weight_elems(self, world: int = 1) -> int:
         d, f, dkv = self.d_model, self.ffn, self.n_kv * self.head_dim
@@ -111,10 +112,13 @@ class LlamaConfig:
         norms = self.layers * 2 * d + d
         kv = self.layers * 2 * self.batch * (self.n_kv // world) * self.head_dim * (pos + 2)
         act = self.layers * 12 * self.batch * d
+        kv_bytes = kv * e
+        if self.kv_fp8:  # one byte per cache element + the 4-byte k / v scale of every KV head
+            kv_bytes = kv + self.layers * 2 * (self.n_kv // world) * 4
         if self.fp8_weights:  # one byte per projection weight + 4 bytes per output column
             cols = self.layers * ((d + 2 * dkv + 2 * f) // world + 2 * d) + self.vocab
-            return proj + 4 * cols + (norms + kv + act) * e
-        return (proj + norms + kv + act) * e
+            return proj + 4 * cols + (norms + act) * e + kv_bytes
+        return (proj + norms + act) * e + kv_bytes
 
 
 @dataclass
@@ -139,6 +143,7 @@ def build_llama_decode(h, cfg: LlamaConfig, world: int = 1, rank: int = 0, seq: 
     assert cfg.n_kv % world == 0 and cfg.heads % cfg.n_kv == 0
     # the FP8 weight GEMM takes at most 64 rows, and a tensor-parallel prompt step is not provided
     assert seq == 1 or (world == 1 and not cfg.fp8_weights), "prompt steps (seq > 1): one GPU, 16-bit weights"
+    assert seq == 1 or not cfg.kv_fp8, "an FP8 KV cache takes one token per step (seq == 1)"
     B, d, H, dh, f, V, dt = cfg.batch, cfg.d_model, cfg.heads // world, cfg.head_dim, cfg.ffn // world, cfg.vocab, cfg.dtype
     Hkv = cfg.n_kv // world
     dl, dkv = H * dh, Hkv * dh  # local attention widths of q and of k / v
@@ -173,12 +178,19 @@ def build_llama_decode(h, cfg: LlamaConfig, world: int = 1, rank: int = 0, seq: 
     x = h.gather(emb, g.input_ids, None, 0)  # [B,seq,d]
     for li in range(cfg.layers):
         p = f"l{li}."
-        kc = h.tensor([B, Hkv, cfg.s_max, dh], dt)
-        vc = h.tensor([B, Hkv, cfg.s_max, dh], dt)
+        kc = h.tensor([B, Hkv, cfg.s_max, dh], FP8 if cfg.kv_fp8 else dt)
+        vc = h.tensor([B, Hkv, cfg.s_max, dh], FP8 if cfg.kv_fp8 else dt)
         kc.set_input()
         vc.set_input()
         g.k_caches.append(kc)
         g.v_caches.append(vc)
+        kv_scales = {}
+        if cfg.kv_fp8:  # per-KV-head f32 scales of this layer's caches, sharded by head with them
+            for which in ("k", "v"):
+                t = h.tensor([Hkv], F32)
+                t.set_weight()
+                g.weights[f"{p}{which}_scale"] = (t, (Hkv,), "kv_scale", ("head", cfg.n_kv))
+                kv_scales[which + "_scale"] = t
         hn = h.RMSNorm(x, weight(p + "ln1", (d,), "norm"), None)
         q = linear(hn, p + "wq", (d, dl), ("col", d))
         k = linear(hn, p + "wk", (d, dkv), ("col", d))
@@ -190,7 +202,7 @@ def build_llama_decode(h, cfg: LlamaConfig, world: int = 1, rank: int = 0, seq: 
             t = h.reshape(t, None, [B, seq, n, dh])
             return h.transpose(t, None, [0, 2, 1, 3])  # [B,n,seq,dh]
 
-        attn = h.attentionKVCache(kc, vc, heads(q), heads(k, Hkv), heads(v, Hkv), g.position_ids, None)
+        attn = h.attentionKVCache(kc, vc, heads(q), heads(k, Hkv), heads(v, Hkv), g.position_ids, None, **kv_scales)
         a = h.reshape(h.transpose(attn, None, [0, 2, 1, 3]), None, [B, seq, dl])
         o = linear(a, p + "wo", (dl, d), ("row", d))
         if world > 1:
@@ -244,7 +256,12 @@ def quantize_fp8_host(w: np.ndarray):
     never imports the oracle): codes uint8 [K, N], scale f32 [N] = max|column| / 448; round to nearest, ties to even."""
     w = np.asarray(w, np.float32)
     scale = np.maximum(np.abs(w).max(axis=0), 1e-12).astype(np.float32) / np.float32(448.0)
-    x = (w / scale[None, :]).astype(np.float32)
+    return e4m3_codes_host((w / scale[None, :]).astype(np.float32)), scale
+
+
+def e4m3_codes_host(x: np.ndarray) -> np.ndarray:
+    """float32 -> FP8 E4M3 codes (uint8): round to nearest, ties to even, saturated to +-448 (finite inputs)."""
+    x = np.asarray(x, np.float32)
     table = np.zeros(127, np.float64)
     for c in range(127):
         e, m = (c >> 3) & 15, c & 7
@@ -254,7 +271,7 @@ def quantize_fp8_host(w: np.ndarray):
     lo = np.clip(hi - 1, 0, 126)
     dlo, dhi = mag - table[lo], table[hi] - mag
     code = np.where((dhi < dlo) | ((dhi == dlo) & (hi % 2 == 0)), hi, lo).astype(np.uint8)
-    return np.where(np.signbit(x), code | 0x80, code).astype(np.uint8), scale
+    return np.where(np.signbit(x), code | 0x80, code).astype(np.uint8)
 
 
 def fill_llama_weights_host(g: LlamaGraph, world: int = 1, rank: int = 0, seed: int = 0):
@@ -262,6 +279,10 @@ def fill_llama_weights_host(g: LlamaGraph, world: int = 1, rank: int = 0, seed: 
     for name, (t, shape, kind, shard) in g.weights.items():
         if kind == "scale":
             continue  # written together with its codes
+        if kind == "kv_scale":  # the scale the cache helpers quantise with (llama_kv_fp8_values)
+            li, which = int(name[1:name.index(".")]), name[name.index(".") + 1]
+            t.copyin_numpy(llama_kv_fp8_values(g.cfg, li, which, world, rank)[1])
+            continue
         if kind == "proj_fp8":
             codes, scale = quantize_fp8_host(llama_weight_values(name, list(shape), "proj", seed))
             t.copyin_numpy(codes)
@@ -280,6 +301,15 @@ def llama_cache_values(cfg: LlamaConfig, layer: int, which: str, world: int = 1,
     full = rng.standard_normal((cfg.batch, cfg.n_kv, cfg.s_max, cfg.head_dim), dtype=np.float32) * np.float32(0.5)
     hl = cfg.n_kv // world
     return np.ascontiguousarray(full[:, rank * hl:(rank + 1) * hl])
+
+
+def llama_kv_fp8_values(cfg: LlamaConfig, layer: int, which: str, world: int = 1, rank: int = 0, seed: int = 2):
+    """llama_cache_values quantised for an FP8 cache (cfg.kv_fp8): scale[h] = max |cache of KV head h| / 448 over the batch,
+    codes = e4m3(value / scale[h]) -- the rule the append applies to new rows.  Returns (codes uint8 [B, Hkv_l, s_max, D],
+    scale f32 [Hkv_l]) for the rank's heads."""
+    x = llama_cache_values(cfg, layer, which, world, rank, seed)
+    scale = (np.maximum(np.abs(x).max(axis=(0, 2, 3)), 1e-12).astype(np.float32) / np.float32(448.0)).astype(np.float32)
+    return e4m3_codes_host(x / scale[None, :, None, None]), scale
 
 
 # ---------------------------------------------------------------- single MatMul (C1)

@@ -30,9 +30,9 @@ from typing import Any, Dict, List, Optional
 import numpy as np
 
 # ONNX TensorProto.DataType codes used by the backend (include/core/data_type.h:6-23 has the same numbering)
-F32, U8, I8, I16, I32, I64, BOOL, F16, F64, U32, BF16 = 1, 2, 3, 5, 6, 7, 9, 10, 11, 12, 16
+F32, U8, I8, I16, I32, I64, BOOL, F16, F64, U32, BF16, FP8 = 1, 2, 3, 5, 6, 7, 9, 10, 11, 12, 16, 17
 _NP = {F32: np.float32, U8: np.uint8, I8: np.int8, I16: np.int16, I32: np.int32, I64: np.int64, BOOL: np.bool_,
-       F16: np.float16, F64: np.float64, U32: np.uint32, BF16: np.uint16}
+       F16: np.float16, F64: np.float64, U32: np.uint32, BF16: np.uint16, FP8: np.uint8}  # FP8: E4M3 "FN" codes
 
 
 # ------------------------------------------------------------------------------------------------ wire format
@@ -549,8 +549,9 @@ class OnnxStub:
                 T[out0] = h.RoPE(I(0), I(1), None, int(a["dim_head"]))
             else:
                 T[out0] = h.RoPE(I(0), I(1), None)
-        elif op == "AttentionKVCache":
-            T[out0] = h.attentionKVCache(I(0), I(1), I(2), I(3), I(4), I(5), None)
+        elif op == "AttentionKVCache":  # optional inputs 6, 7 (extension): k_scale / v_scale of FP8 E4M3 caches
+            scales = {"k_scale": I(6), "v_scale": I(7)} if len(nd.inputs) > 6 else {}
+            T[out0] = h.attentionKVCache(I(0), I(1), I(2), I(3), I(4), I(5), None, **scales)
         elif op in ("MaxPool", "AveragePool"):
             k = a["kernel_shape"]
             d, p, s = a.get("dilations", [1, 1]), list(a.get("pads", [0, 0, 0, 0])), a.get("strides", [1, 1])
@@ -750,9 +751,12 @@ class OnnxExporter:
         return self._emit("RoPE", [pos, x], self.inner.RoPE(pos.inner, x.inner, self._in(y), *extra),
                           {"dim_head": extra[0]} if extra else None)
 
-    def attentionKVCache(self, kc, vc, q, k, v, pos, y):
-        r = self.inner.attentionKVCache(kc.inner, vc.inner, q.inner, k.inner, v.inner, pos.inner, self._in(y))
-        return self._emit("AttentionKVCache", [kc, vc, q, k, v, pos], r)
+    def attentionKVCache(self, kc, vc, q, k, v, pos, y, k_scale=None, v_scale=None):
+        # the FP8 caches' scales only when given: every 16-bit export stays as it was
+        scales = [] if k_scale is None else [k_scale, v_scale]
+        r = self.inner.attentionKVCache(kc.inner, vc.inner, q.inner, k.inner, v.inner, pos.inner, self._in(y),
+                                        **({"k_scale": k_scale.inner, "v_scale": v_scale.inner} if scales else {}))
+        return self._emit("AttentionKVCache", [kc, vc, q, k, v, pos] + scales, r)
 
     def _pool(self, op, fn, x, y, kh, kw, dh, dw, ph, pw, sh, sw, ceil):
         r = fn(x.inner, self._in(y), kh, kw, dh, dw, ph, pw, sh, sw, ceil)
@@ -1030,6 +1034,20 @@ def parallel_model(model, world: int, rank: int, new_handler=None) -> Model:
                     v = inputs[cache]
                     inputs[cache] = ValueInfo(v.name, v.elem_type, [d // world if i == 1 else d for i, d in enumerate(v.dims)])
                     place[cache] = 1
+            for i in (6, 7):  # an FP8 cache's per-KV-head scales split with its heads
+                if i >= len(nd.inputs) or place.get(nd.inputs[i]) == 0:
+                    continue
+                sc = nd.inputs[i]
+                if sc in consts:
+                    c = consts[sc]
+                    nd.inputs[i] = new_const(c.name, shard_array(c.array, 0), c.data_type)
+                    place[nd.inputs[i]] = 0
+                elif sc in inputs:
+                    v = inputs[sc]
+                    inputs[sc] = ValueInfo(v.name, v.elem_type, [v.dims[0] // world])
+                    place[sc] = 0
+                else:
+                    raise NotImplementedError("AttentionKVCache: k_scale / v_scale must be graph inputs or initializers")
             place[nd.outputs[0]] = 1
         elif op == "MatMul":
             a_ax, b_ax = place.get(nd.inputs[0]), place.get(nd.inputs[1])
