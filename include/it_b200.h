@@ -202,6 +202,28 @@ int it_b200_matmul_fp8w(int dtype, const void *X, int n_groups, const void *cons
 int it_b200_dequantize_fp8(int dtype_out, const void *xq, const float *scale, void *y, int64_t rows, int64_t cols,
                            void *stream);
 
+/* ---- Weight-only 4-bit MatMul: the subset of ONNX com.microsoft MatMulNBits this project accepts (no counterpart in the reference).
+ *      C_i[m, N_i] = X[m, K] . W_i,   W[k, n] = (q[n, k] - z[n, k / bs]) * s[n, k / bs],   bs = block_size in {32, 64, 128}.
+ *      X, C, s and the residual: f16 or bf16, all of the same dtype (fp32 is refused).
+ *      Wq_i (MatMulNBits input B): uint8 [N, K / bs, bs / 2], N-major -- column n's K codes are K / 2 contiguous bytes; element k of
+ *           column n is in byte (n, k / bs, (k % bs) / 2), even k in the low nibble, odd k in the high nibble.
+ *      scales_i: [N * K / bs] of the activation dtype; the scale of (n, block) is element n * (K / bs) + block.
+ *      zero_points: NULL (z = 8 everywhere) or one pointer per matrix, uint8 nibble-packed: (K / bs) / 2 bytes per column, block b
+ *           at byte n * (K / bs) / 2 + b / 2, low nibble for even b.  Accepted only when K / bs is even.
+ *      K % bs == 0, N_i % 16 == 0; X, Wq_i, C_i and the residual 16-byte aligned.  1..4 matrices sharing X; residual (single
+ *      matrix only, may be NULL) is added after the product has been rounded to the dtype, like MatMul -> Add.
+ *      m <= 64: gemm_skinny_w4_kernel.  (q - z) enters the tensor core exactly in the activation type; each block's fp32 partial
+ *           sum is multiplied by fp32(s) and added to the fp32 accumulator; the output is rounded once.  No workspace.
+ *      m > 64: each matrix is dequantised to T((q - z) * s) [K, N] in the workspace (it_b200_matmul_nbits_workspace bytes),
+ *           then multiplied by it_b200_matmul: the weights are rounded to the dtype once, unlike the decode kernel.
+ *      it_b200_dequantize_w4 is that dequantiser on its own: W [K, N] row-major = T((q - z) * s), the product in fp32. ---- */
+int64_t it_b200_matmul_nbits_workspace(int dtype, int m, int k, int n_groups, const int *N);
+int it_b200_matmul_nbits(int dtype, const void *X, int n_groups, const void *const *Wq, const void *const *scales,
+                         const void *const *zero_points, void *const *C, const int *N, int m, int k, int block_size,
+                         const void *residual, void *workspace, int64_t workspace_bytes, void *stream);
+int it_b200_dequantize_w4(int dtype, const void *Wq, const void *scales, const void *zero_points, void *W, int k, int n,
+                          int block_size, void *stream);
+
 /* ---- SiLU(gate) * up in one pass (the fused form of Silu -> Mul; the Silu result is rounded to the storage
  *      dtype before the multiply, exactly as the two separate kernels would). ---- */
 int it_b200_silu_mul(int dtype, const void *gate, const void *up, void *out, int64_t n, void *stream);

@@ -64,6 +64,10 @@ _SIGS = {
     "it_b200_silu_mul": (c_int, [c_int, vp, vp, vp, c_int64, vp]),
     "it_b200_matmul_fp8w": (c_int, [c_int, vp, c_int, POINTER(vp), POINTER(vp), POINTER(vp), i32p, c_int, c_int, vp, vp]),
     "it_b200_dequantize_fp8": (c_int, [c_int, vp, vp, vp, c_int64, c_int64, vp]),
+    "it_b200_matmul_nbits_workspace": (c_int64, [c_int, c_int, c_int, c_int, i32p]),
+    "it_b200_matmul_nbits": (c_int, [c_int, vp, c_int, POINTER(vp), POINTER(vp), POINTER(vp), POINTER(vp), i32p, c_int, c_int, c_int,
+                                     vp, vp, c_int64, vp]),
+    "it_b200_dequantize_w4": (c_int, [c_int, vp, vp, vp, vp, c_int, c_int, c_int, vp]),
     "it_b200_allreduce_workspace_bytes": (c_int64, []),
     "it_b200_allreduce_fused": (c_int, [c_int, vp, vp, vp, vp, vp, c_int, c_int, POINTER(vp), c_int, c_int, vp, vp]),
     "it_b200_batchnorm_relu": (c_int, [c_int, vp, vp, vp, vp, vp, vp, c_int, c_int, c_int64, c_float, vp]),

@@ -354,6 +354,15 @@ class GraphHandler:
         ins = [a, b] + ([bias] if bias is not None else []) + ([w_scale] if w_scale is not None else [])
         return self._op1("MatMul", ins, y, [int(transA), int(transB), int(act), 1 if w_scale is not None else 0])
 
+    def matMulNBits(self, a, b, scales, zero_points, y, K, N, block_size, bits=4, g_idx=None, bias=None):
+        """com.microsoft MatMulNBits (extension), 4-bit weights with block-wise scales: y[.., N] = a[.., K] . W,
+        W[k, n] = (q[n, k] - z[n, k // block_size]) * scales[n * (K // block_size) + k // block_size].  b: uint8 [N, K // bs, bs // 2]
+        (even k in the low nibble); zero_points: None (z = 8) or uint8 nibble-packed [N * (K // bs) // 2].  a / scales / y: f16 or bf16.
+        g_idx and bias are the operator's optional inputs; the backend refuses them."""
+        opt = [zero_points, g_idx, bias]
+        ins = [a, b, scales] + [t for t in opt if t is not None]
+        return self._op1("MatMulNBits", ins, y, [int(K), int(N), int(bits), int(block_size)] + [int(t is not None) for t in opt])
+
     def batchNormalization(self, input, output, mean, var, scale, bias, momentum, eps, training):
         return self._op1("BatchNormalization", [input, mean, var, scale, bias], output, [int(training)], [momentum, eps])
 

@@ -358,7 +358,41 @@ namespace b200 {
 // MatMul with optional fused residual: C = A.B (+ bias) ; when `residual` is given (MatMul -> Add fusion) the
 // product is rounded to the storage dtype first, the residual added in the epilogue and the result written to
 // `outOverride` (the Add's output) -- bit-identical to the two separate kernels.
+#ifndef ITB_SEAM_A
+// MatMulNBits: 1..4 operators sharing A (a MatMulGroup step, grouped like with like by the schedule) in one it_b200_matmul_nbits call;
+// `residual` / `outOverride` as for runMatmul (single operator)
+static void runMatmulNBits(const OpVec &ops, const RuntimeObj *ctx, const Tensor &residual, const Tensor &outOverride) {
+    IT_ASSERT(!ops.empty() && ops.size() <= 4);
+    auto op0 = as<MatMulNBitsObj>(ops[0]);
+    auto A = op0->getInputs(0);
+    const int k = op0->getK();
+    const int rows = (int)(A->size() / k);
+    const bool zp = op0->getZeroPoints() != nullptr;
+    const void *W[4], *Sc[4], *Z[4];
+    void *C[4];
+    int N[4];
+    for (size_t i = 0; i < ops.size(); ++i) {
+        auto op = as<MatMulNBitsObj>(ops[i]);
+        IT_ASSERT(op->getInputs(0) == A && op->getBlockSize() == op0->getBlockSize() && (op->getZeroPoints() != nullptr) == zp,
+                  "MatMulNBits group: one activation, block size and zero-point presence");
+        W[i] = P(op->getInputs(1));
+        Sc[i] = P(op->getInputs(2));
+        Z[i] = zp ? P(op->getZeroPoints()) : nullptr;
+        C[i] = P(outOverride ? outOverride : op->getOutput());
+        N[i] = op->getN();
+    }
+    const int ng = (int)ops.size();
+    const int64_t wsb = it_b200_matmul_nbits_workspace(DTI(A), rows, k, ng, N);
+    void *ws = wsb ? RT(ctx)->getWorkspace((size_t)wsb) : nullptr;
+    CK(it_b200_matmul_nbits(DTI(A), P(A), ng, W, Sc, zp ? Z : nullptr, C, N, rows, k, op0->getBlockSize(),
+                            residual ? P(residual) : nullptr, ws, wsb, S()), ops[0]);
+}
+#endif
+
 void runMatmul(const Operator &_op, const RuntimeObj *ctx, const Tensor &residual, const Tensor &outOverride) {
+#ifndef ITB_SEAM_A
+    if (_op->getOpType() == OpType::MatMulNBits) return runMatmulNBits({_op}, ctx, residual, outOverride);
+#endif
     auto op = as<MatmulObj>(_op);
     auto A = op->getInputs(0), B = op->getInputs(1);
     auto C = outOverride ? outOverride : op->getOutput();
@@ -434,7 +468,8 @@ void runMatmul(const Operator &_op, const RuntimeObj *ctx, const Tensor &residua
 // MatMul (+ bias) -> [Gelu] -> [Add(residual)]: ops = {MatMul, [Gelu], [Add]} in one wgmma epilogue.  false = the shape is not
 // taken (nothing launched): the caller runs the operators one by one.
 bool matmulAddIsPlain(const OpVec &ops) {
-    return ops.size() == 2 && ops[1]->getOpType() == OpType::Add && !as<MatmulObj>(ops[0])->getBias();
+    if (ops.size() != 2 || ops[1]->getOpType() != OpType::Add) return false;
+    return ops[0]->getOpType() == OpType::MatMulNBits || !as<MatmulObj>(ops[0])->getBias();
 }
 bool runMatmulFused(const OpVec &ops, const RuntimeObj *) {
     auto mm = as<MatmulObj>(ops[0]);
@@ -469,7 +504,8 @@ bool runMatmulFused(const OpVec &ops, const RuntimeObj *) {
 }
 
 // q/k/v or gate/up: MatMuls sharing the activation operand, weights [K, N_i]: one grouped launch
-void runMatmulGroup(const OpVec &ops, const RuntimeObj *) {
+void runMatmulGroup(const OpVec &ops, const RuntimeObj *ctx) {
+    if (ops[0]->getOpType() == OpType::MatMulNBits) return runMatmulNBits(ops, ctx, nullptr, nullptr);
     auto A = ops[0]->getInputs(0);
     int k = as<MatmulObj>(ops[0])->getK();
     int64_t rows = 1;
@@ -759,6 +795,11 @@ class MatmulB200 : public CudaKernelWithoutConfig {
     }
 #endif
 };
+#ifndef ITB_SEAM_A
+class MatMulNBitsB200 : public CudaKernelWithoutConfig {
+    void compute(const Operator &op, const RuntimeObj *ctx) const override { b200::runMatmul(op, ctx, nullptr, nullptr); }
+};
+#endif
 class ConvB200 : public CudaKernelWithoutConfig {
     void compute(const Operator &_op, const RuntimeObj *ctx) const override {
         auto op = as<ConvObj>(_op);
@@ -918,6 +959,7 @@ REG(MatMul, MatmulB200, "Matmul_B200_tma")  // decode shapes: TMA + mma.sync (ge
 REG(Conv, ConvB200, "Conv_B200_im2col_gemm")
 REG(AttentionKVCache, AttentionKVCacheB200, "AttentionKVCache_B200")
 #ifndef ITB_SEAM_A
+REG(MatMulNBits, MatMulNBitsB200, "MatMulNBits_B200")  // m <= 64: gemm_skinny_w4_kernel; more rows: dequantise + the 16-bit GEMM
 REG(AllReduceSum, AllReduceB200, "AllReduceSum_B200")
 REG(AllReduceProd, AllReduceB200, "AllReduceProd_B200")
 REG(AllReduceMin, AllReduceB200, "AllReduceMin_B200")

@@ -232,6 +232,21 @@ static Operator build_op(itb_graph *h, const string &name, const TensorVec &in, 
         return g->addOp<MatmulObj>(in[0], in[1], o0, (bool)I(0), (bool)I(1), nb > 2 ? in[2] : nullptr, (ActType)I(2), "default",
                                    scaled ? in.back() : nullptr);
     }
+    case OpType::MatMulNBits:
+    {
+        // inputs A, B, scales, then the optional zero_points, g_idx, bias that are present; iattrs K, N, bits, block_size and
+        // one presence flag per optional input
+        need(3);
+        size_t next = 3;
+        auto opt = [&](int flag) -> Tensor {
+            if (!I(flag)) return nullptr;
+            need(next + 1);
+            return in[next++];
+        };
+        Tensor zp = opt(4), gidx = opt(5), bias = opt(6);
+        IT_ASSERT(next == in.size(), "MatMulNBits: " + std::to_string(in.size()) + " inputs do not match the presence flags");
+        return g->addOp<MatMulNBitsObj>(in[0], in[1], in[2], zp, o0, (int)I(0), (int)I(1), (int)I(2, 4), (int)I(3), gidx, bias);
+    }
     case OpType::Conv:
         need(2);
         return g->addOp<ConvObj>(in[0], in[1], o0, (int)I(0), (int)I(1), (int)I(2, 1), (int)I(3, 1), (int)I(4, 1),

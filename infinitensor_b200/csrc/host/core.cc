@@ -24,7 +24,7 @@ static const char *kOpNames[] = {
     "DepthToSpace", "Div", "Elu", "Equal", "Erf", "Exp", "Expand", "Flatten", "Gather", "Gelu", "Greater", "HardSigmoid",
     "HardSwish", "Identity", "LayerNormalization", "LeakyRelu", "Less", "MatMul", "Max", "MaxPool", "Min", "Mul", "Neg", "Pad",
     "Pow", "RMSNorm", "ReduceMean", "ReduceSum", "Relu", "Reshape", "RoPE", "Sigmoid", "Silu", "Slice", "Softmax",
-    "Split", "Sqrt", "Squeeze", "Sub", "Tanh", "Transpose", "Unsqueeze", "Where"};
+    "Split", "Sqrt", "Squeeze", "Sub", "Tanh", "Transpose", "Unsqueeze", "Where", "MatMulNBits"};
 static_assert(sizeof(kOpNames) / sizeof(kOpNames[0]) == OpType::NumOpTypes, "op name table out of sync");
 
 const char *OpType::toString() const { return type < NumOpTypes ? kOpNames[type] : "Unknown"; }

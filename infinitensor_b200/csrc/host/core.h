@@ -90,7 +90,9 @@ struct OpType {
         AttentionKVCache, AveragePool, BatchNormalization, Cast, Concat, Conv, DepthToSpace, Div, Elu, Equal, Erf, Exp,
         Expand, Flatten, Gather, Gelu, Greater, HardSigmoid, HardSwish, Identity, LayerNormalization, LeakyRelu, Less, MatMul,
         Max, MaxPool, Min, Mul, Neg, Pad, Pow, RMSNorm, ReduceMean, ReduceSum, Relu, Reshape, RoPE, Sigmoid, Silu,
-        Slice, Softmax, Split, Sqrt, Squeeze, Sub, Tanh, Transpose, Unsqueeze, Where, NumOpTypes
+        Slice, Softmax, Split, Sqrt, Squeeze, Sub, Tanh, Transpose, Unsqueeze, Where,
+        MatMulNBits,  // (extensions after the reference's alphabetical list, so that its numbering stays)
+        NumOpTypes
     } type;
     constexpr OpType(decltype(type) t = Unknown) : type(t) {}
     constexpr explicit OpType(underlying_t v) : type((decltype(type))v) {}

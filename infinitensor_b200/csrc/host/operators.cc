@@ -55,6 +55,52 @@ vector<int> MatmulObj::getWorkloadVector() const {
     return {(int)type.underlying(), b, m, n, k, transA, transB, (int)act, inputs[0]->getDTypeIndex()};
 }
 
+// ---------------------------------------------------------------- MatMulNBits (extension)
+static TensorVec nbitsInputs(Tensor A, Tensor B, Tensor scales, Tensor zp) {
+    TensorVec v{A, B, scales};
+    if (zp) v.push_back(zp);
+    return v;
+}
+MatMulNBitsObj::MatMulNBitsObj(GraphObj *graph, Tensor A, Tensor B, Tensor scales, Tensor zeroPoints, Tensor Y, int K, int N, int bits,
+                               int blockSize, Tensor gIdx, Tensor bias)
+    : OperatorObj(OpType::MatMulNBits, nbitsInputs(A, B, scales, zeroPoints), {Y}), K(K), N(N), bits(bits), blockSize(blockSize) {
+    IT_ASSERT(bits == 4, "MatMulNBits: bits = " + std::to_string(bits) + "; only 4-bit weights are supported");
+    IT_ASSERT(blockSize == 32 || blockSize == 64 || blockSize == 128,
+              "MatMulNBits: block_size = " + std::to_string(blockSize) + " is not 32, 64 or 128");
+    IT_ASSERT(K > 0 && K % blockSize == 0,
+              "MatMulNBits: K = " + std::to_string(K) + " is not a positive multiple of block_size " + std::to_string(blockSize));
+    IT_ASSERT(N > 0 && N % 16 == 0, "MatMulNBits: N = " + std::to_string(N) + " is not a positive multiple of 16");
+    IT_ASSERT(!gIdx, "MatMulNBits: the g_idx input (act-order) is not supported");
+    IT_ASSERT(!bias, "MatMulNBits: the bias input is not supported");
+    const auto dt = A->getDType();
+    IT_ASSERT(dt != DataType::Float32, "MatMulNBits: fp32 activations are not supported (f16 / bf16 only)");
+    IT_ASSERT(dt == DataType::Float16 || dt == DataType::BFloat16, "MatMulNBits: A must be f16 or bf16, not " + dt.toString());
+    const int nblk = K / blockSize;
+    IT_ASSERT(B->getDType() == DataType::UInt8 && B->getDims() == Shape({N, nblk, blockSize / 2}),
+              "MatMulNBits: B must be uint8 [N, K / block_size, block_size / 2] = " + vecToString(Shape({N, nblk, blockSize / 2})) +
+                  ", got " + B->getDType().toString() + " " + vecToString(B->getDims()));
+    IT_ASSERT(scales->getDType() == dt && (int64_t)scales->size() == (int64_t)N * nblk,
+              "MatMulNBits: scales must hold N * K / block_size = " + std::to_string((int64_t)N * nblk) + " values of A's dtype");
+    if (zeroPoints) {
+        IT_ASSERT(nblk % 2 == 0, "MatMulNBits: zero points need an even number of blocks per column (K / block_size = " +
+                                     std::to_string(nblk) + ")");
+        IT_ASSERT(zeroPoints->getDType() == DataType::UInt8 && (int64_t)zeroPoints->size() == (int64_t)N * nblk / 2,
+                  "MatMulNBits: zero_points must be uint8 with N * (K / block_size) / 2 = " + std::to_string((int64_t)N * nblk / 2) +
+                      " packed bytes");
+    }
+    IT_ASSERT(checkValid(graph));
+}
+std::optional<vector<Shape>> MatMulNBitsObj::inferShape(const TensorVec &ins) {
+    Shape s = ins[0]->getDims();
+    IT_ASSERT(!s.empty() && s.back() == K, "MatMulNBits: the last dimension of A must be K = " + std::to_string(K));
+    s.back() = N;
+    return {{s}};
+}
+vector<int> MatMulNBitsObj::getWorkloadVector() const {
+    int rows = (int)(inputs[0]->size() / K);
+    return {(int)type.underlying(), rows, N, K, blockSize, (int)inputs.size(), inputs[0]->getDTypeIndex()};
+}
+
 // ---------------------------------------------------------------- Conv (src/operators/conv.cc:85-114)
 ConvObj::ConvObj(GraphObj *graph, Tensor input, Tensor weight, Tensor output, int ph, int pw, int sh, int sw,
                  int dh, int dw, Tensor bias, ActType act)

@@ -40,6 +40,27 @@ class MatmulObj : public OperatorObj {
     string getComputeType() const { return computeType; }
 };
 
+// com.microsoft MatMulNBits with bits = 4 (extension; the reference has no quantised MatMul): Y[.., N] = A[.., K] . W,
+// W[k, n] = (q[n, k] - z[n, k / bs]) * s[n, k / bs].  Inputs: A (f16 / bf16), B uint8 [N, K / bs, bs / 2] (column n's codes contiguous,
+// even k in the low nibble), scales [N * K / bs] of A's dtype, optional zero_points uint8 [N * (K / bs) / 2] (nibble-packed, low
+// nibble for even blocks; only when K / bs is even; absent: z = 8).  The layout is spelled out in it_b200.h (it_b200_matmul_nbits).
+class MatMulNBitsObj : public OperatorObj {
+    int K, N, bits, blockSize;
+
+  public:
+    // gIdx / bias: the operator's optional inputs 4 and 5, refused when present
+    MatMulNBitsObj(GraphObj *graph, Tensor A, Tensor B, Tensor scales, Tensor zeroPoints, Tensor Y, int K, int N, int bits, int blockSize,
+                   Tensor gIdx = nullptr, Tensor bias = nullptr);
+    std::optional<vector<Shape>> inferShape(const TensorVec &inputs) override;
+    vector<DataType> inferDataType(const TensorVec &ins) const override { return {ins[0]->getDType()}; }
+    vector<int> getOpAttrVector() const override { return {(int)type.underlying(), K, N, bits, blockSize, (int)inputs.size()}; }
+    vector<int> getWorkloadVector() const override;
+    Tensor getZeroPoints() const { return inputs.size() > 3 ? inputs[3] : nullptr; }
+    int getK() const { return K; }
+    int getN() const { return N; }
+    int getBlockSize() const { return blockSize; }
+};
+
 class ConvObj : public OperatorObj {
     int ph, pw, sh, sw, dh, dw;
     ActType act;

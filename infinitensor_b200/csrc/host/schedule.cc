@@ -403,7 +403,7 @@ const vector<ExecStep> &GraphObj::getSchedule() {
                 schedule.push_back(std::move(st));
                 continue;
             }
-            st.kind = pt == OpType::MatMul ? ExecStep::MatMulAdd : pt == OpType::Silu ? ExecStep::SiluMul : ExecStep::AllReduceAddNorm;
+            st.kind = pt == OpType::MatMul || pt == OpType::MatMulNBits ? ExecStep::MatMulAdd : pt == OpType::Silu ? ExecStep::SiluMul : ExecStep::AllReduceAddNorm;
             st.ops = prod;  // MatMulAdd: {MatMul, [activation], Add | activation}; the others: one producer
             st.ops.push_back(op);
             if (st.kind == ExecStep::AllReduceAddNorm) {
@@ -493,6 +493,44 @@ const vector<ExecStep> &GraphObj::getSchedule() {
                     chain.pop_back();
                     deferredInto[last.get()] = chain;
                     for (auto &m : chain) deferred.insert(m.get());
+                    continue;
+                }
+            }
+        } else if (type == OpType::MatMulNBits) {
+            // the 4-bit MatMul takes the same two fusions as the 16-bit one: (1) later MatMulNBits reading the same activation with
+            // the same K, block size and zero-point presence, in the decode regime, run as one grouped launch; (2) MatMulNBits ->
+            // Add(residual of identical shape) runs at the Add's position with the residual added after the product is rounded
+            auto nb = as<MatMulNBitsObj>(op);
+            auto A = op->getInputs(0);
+            auto like = [&](const Operator &c) {
+                auto o = as<MatMulNBitsObj>(c);
+                return o && c->getInputs(0) == A && o->getK() == nb->getK() && o->getBlockSize() == nb->getBlockSize() &&
+                       (o->getZeroPoints() != nullptr) == (nb->getZeroPoints() != nullptr);
+            };
+            if ((mask & 2) && rowsOf(A) <= 64) {
+                for (auto &cand : A->getTargets()) {
+                    if (st.ops.size() >= 4) break;
+                    if (cand == op || consumed.count(cand.get()) || deferred.count(cand.get()) || pos[cand.get()] < (int)i) continue;
+                    if (like(cand)) st.ops.push_back(cand);
+                }
+                if (st.ops.size() > 1) {
+                    st.kind = ExecStep::MatMulGroup;
+                    std::sort(st.ops.begin(), st.ops.end(),
+                              [&](const Operator &a, const Operator &b) { return pos[a.get()] < pos[b.get()]; });
+                    for (size_t j = 1; j < st.ops.size(); ++j) consumed.insert(st.ops[j].get());
+                }
+            }
+            auto out = op->getOutput();
+            auto targets = out->getTargets();
+            if (st.kind == ExecStep::Single && (mask & 4) && targets.size() == 1 && !out->isOutput() &&
+                targets[0]->getOpType() == OpType::Add && !deferredInto.count(targets[0].get()) && !deferred.count(targets[0].get()) &&
+                !consumed.count(targets[0].get())) {
+                auto add = targets[0];
+                auto other = add->getInputs(0) == out ? add->getInputs(1) : add->getInputs(0);
+                if (other != out && other->getDims() == out->getDims() && other->getDType() == out->getDType() &&
+                    add->getOutput()->getDims() == out->getDims()) {
+                    deferredInto[add.get()] = {op};
+                    deferred.insert(op.get());
                     continue;
                 }
             }

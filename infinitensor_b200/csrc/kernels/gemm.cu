@@ -60,6 +60,21 @@ bool make_tma_2d_u8(CUtensorMap *map, const void *base, uint64_t rows, uint64_t 
     return r == CUDA_SUCCESS;
 }
 
+// the same over bytes with 128B swizzle (box_cols = 128: the 4-bit codes of gemm_w4.cu, one 128-byte row per output column)
+bool make_tma_2d_u8_sw128(CUtensorMap *map, const void *base, uint64_t rows, uint64_t cols, uint64_t row_stride_bytes,
+                          uint32_t box_rows, uint32_t box_cols) {
+    auto fn = get_encode_fn();
+    if (!fn) return false;
+    cuuint64_t gdim[2] = {cols, rows};
+    cuuint64_t gstride[1] = {row_stride_bytes};
+    cuuint32_t box[2] = {box_cols, box_rows};
+    cuuint32_t estr[2] = {1, 1};
+    CUresult r = fn(map, CU_TENSOR_MAP_DATA_TYPE_UINT8, 2, const_cast<void *>(base), gdim, gstride, box, estr,
+                    CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                    CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    return r == CUDA_SUCCESS;
+}
+
 // 3-D tensor [batch][rows][cols] of 2-byte elements (batch stride in elements), box [1, box_rows, box_cols], 128B swizzle
 bool make_tma_3d_b16(CUtensorMap *map, const void *base, uint64_t batch, uint64_t rows, uint64_t cols,
                      uint64_t row_stride_elems, uint64_t batch_stride_elems, uint32_t box_rows, uint32_t box_cols) {

@@ -67,6 +67,9 @@ bool make_tma_2d_b16(CUtensorMap *map, const void *base, uint64_t rows, uint64_t
 // 2-D row-major tensor [rows, cols] of BYTES (fp8 codes), box [box_rows, box_cols], no swizzle
 bool make_tma_2d_u8(CUtensorMap *map, const void *base, uint64_t rows, uint64_t cols, uint64_t row_stride_bytes,
                     uint32_t box_rows, uint32_t box_cols);
+// the same with 128B swizzle (box_cols = 128)
+bool make_tma_2d_u8_sw128(CUtensorMap *map, const void *base, uint64_t rows, uint64_t cols, uint64_t row_stride_bytes,
+                          uint32_t box_rows, uint32_t box_cols);
 
 bool make_tma_3d_b16(CUtensorMap *map, const void *base, uint64_t batch, uint64_t rows, uint64_t cols,
                      uint64_t row_stride_elems, uint64_t batch_stride_elems, uint32_t box_rows, uint32_t box_cols);

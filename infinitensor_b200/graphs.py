@@ -23,6 +23,7 @@ import numpy as np
 
 F32, F16, BF16, I64, I32 = 1, 10, 16, 7, 6
 FP8 = 17  # FP8 E4M3 codes: weights (SURVEY 8(f-4)) and, with LlamaConfig.kv_fp8, the KV caches
+U8 = 2  # packed 4-bit weight codes (LlamaConfig.int4_block)
 LINEAR = 0
 
 
@@ -77,16 +78,17 @@ class LlamaConfig:
     fp8_weights: bool = False  # the seven projection matrices of every layer + the logits head as FP8 E4M3 codes + f32 column scales
     kv_heads: int | None = None  # grouped-query attention: KV heads shared by heads // kv_heads query heads each; None = heads
     kv_fp8: bool = False  # KV caches as FP8 E4M3 codes + per-layer f32 [KV heads] k / v scales (one token per step)
+    int4_block: int = 0  # 32 / 64 / 128: the seven projections of every layer + the logits head as MatMulNBits (4-bit, symmetric)
 
     @property
     def n_kv(self) -> int:
         return self.heads if self.kv_heads is None else self.kv_heads
 
     @staticmethod
-    def llama3_8b(batch=16, s_max=1024, dtype=BF16, layers=32, kv_fp8=False):
+    def llama3_8b(batch=16, s_max=1024, dtype=BF16, layers=32, kv_fp8=False, int4_block=0):
         """Llama-3-8B shape: 32 query heads over 8 KV heads (G = 4)."""
         return LlamaConfig(layers=layers, d_model=4096, heads=32, kv_heads=8, head_dim=128, ffn=14336, vocab=128256,
-                           s_max=s_max, batch=batch, dtype=dtype, kv_fp8=kv_fp8)
+                           s_max=s_max, batch=batch, dtype=dtype, kv_fp8=kv_fp8, int4_block=int4_block)
 
     @staticmethod
     def tiny(dtype=BF16, layers=2, batch=4, kv_fp8=False):
@@ -94,10 +96,10 @@ class LlamaConfig:
                            batch=batch, dtype=dtype, kv_fp8=kv_fp8)
 
     @staticmethod
-    def tinyllama_1b(batch=16, s_max=1024, dtype=BF16, layers=22, kv_fp8=False):
+    def tinyllama_1b(batch=16, s_max=1024, dtype=BF16, layers=22, kv_fp8=False, int4_block=0):
         """TinyLlama-1.1B shape: 32 query heads of 64 over 4 KV heads (G = 8)."""
         return LlamaConfig(layers=layers, d_model=2048, heads=32, kv_heads=4, head_dim=64, ffn=5632, vocab=32000,
-                           s_max=s_max, batch=batch, dtype=dtype, kv_fp8=kv_fp8)
+                           s_max=s_max, batch=batch, dtype=dtype, kv_fp8=kv_fp8, int4_block=int4_block)
 
     def weight_elems(self, world: int = 1) -> int:
         d, f, dkv = self.d_model, self.ffn, self.n_kv * self.head_dim
@@ -115,6 +117,8 @@ class LlamaConfig:
         kv_bytes = kv * e
         if self.kv_fp8:  # one byte per cache element + the 4-byte k / v scale of every KV head
             kv_bytes = kv + self.layers * 2 * (self.n_kv // world) * 4
+        if self.int4_block:  # half a byte per projection weight + one 16-bit scale per block of int4_block weights
+            return proj // 2 + 2 * (proj // self.int4_block) + (norms + act) * e + kv_bytes
         if self.fp8_weights:  # one byte per projection weight + 4 bytes per output column
             cols = self.layers * ((d + 2 * dkv + 2 * f) // world + 2 * d) + self.vocab
             return proj + 4 * cols + (norms + act) * e + kv_bytes
@@ -144,6 +148,13 @@ def build_llama_decode(h, cfg: LlamaConfig, world: int = 1, rank: int = 0, seq: 
     # the FP8 weight GEMM takes at most 64 rows, and a tensor-parallel prompt step is not provided
     assert seq == 1 or (world == 1 and not cfg.fp8_weights), "prompt steps (seq > 1): one GPU, 16-bit weights"
     assert seq == 1 or not cfg.kv_fp8, "an FP8 KV cache takes one token per step (seq == 1)"
+    if cfg.int4_block:
+        if cfg.int4_block not in (32, 64, 128):
+            raise ValueError(f"int4_block = {cfg.int4_block}: 32, 64 or 128")
+        if world > 1:
+            raise ValueError("int4 weights (int4_block): tensor-parallel sharding is not provided; world must be 1")
+        if cfg.fp8_weights:
+            raise ValueError("int4_block and fp8_weights exclude each other")
     B, d, H, dh, f, V, dt = cfg.batch, cfg.d_model, cfg.heads // world, cfg.head_dim, cfg.ffn // world, cfg.vocab, cfg.dtype
     Hkv = cfg.n_kv // world
     dl, dkv = H * dh, Hkv * dh  # local attention widths of q and of k / v
@@ -158,7 +169,18 @@ def build_llama_decode(h, cfg: LlamaConfig, world: int = 1, rank: int = 0, seq: 
         return t
 
     def linear(x_, name, shape, shard=None):
-        """x . W: 16-bit weight, or (cfg.fp8_weights) FP8 E4M3 codes + per-column f32 scale dequantised inside the GEMM"""
+        """x . W: 16-bit weight, or (cfg.fp8_weights) FP8 E4M3 codes + per-column f32 scale dequantised inside the GEMM, or
+        (cfg.int4_block) MatMulNBits: 4-bit codes [N, K / bs, bs / 2] + one scale of the activation type per block of bs"""
+        if cfg.int4_block:
+            K_, N_ = shape
+            bs = cfg.int4_block
+            wq = h.tensor([N_, K_ // bs, bs // 2], U8)
+            wq.set_weight()
+            sc = h.tensor([N_ * (K_ // bs)], dt)
+            sc.set_weight()
+            g.weights[name] = (wq, tuple(shape), "proj_int4", shard)
+            g.weights[name + ".scale"] = (sc, (N_ * (K_ // bs),), "scale", None)
+            return h.matMulNBits(x_, wq, sc, None, None, K_, N_, bs)
         if not cfg.fp8_weights:
             return h.matmul(x_, weight(name, shape, "proj", shard), None, False, False, None, LINEAR)
         assert world == 1, "fp8 weights: single GPU"
@@ -274,6 +296,23 @@ def e4m3_codes_host(x: np.ndarray) -> np.ndarray:
     return np.where(np.signbit(x), code | 0x80, code).astype(np.uint8)
 
 
+def quantize_w4(w: np.ndarray, block: int, dtype: int = BF16):
+    """Symmetric 4-bit block quantisation of W [K, N] in MatMulNBits' layout (no zero points, so z = 8): per column n and block b
+    of `block` consecutive k, scale = amax / 7 rounded to the activation dtype, q = clamp(rint(w / scale) + 8, 0, 15), rint
+    rounding half to even.  Returns (codes uint8 [N, K / block, block / 2] with even k in the low nibble, scale float32 [N * K / block]
+    holding values exact in `dtype`)."""
+    w = np.asarray(w, np.float32)
+    K, N = w.shape
+    assert K % block == 0
+    wb = w.T.reshape(N, K // block, block)
+    amax = np.abs(wb).max(axis=2)
+    scale = from_storage(to_storage(amax / np.float32(7.0), dtype), dtype).astype(np.float32)
+    safe = np.where(scale > 0, scale, np.float32(1.0))
+    q = np.clip(np.rint(wb / safe[:, :, None]) + 8, 0, 15).astype(np.uint8)
+    codes = (q[:, :, 0::2] | (q[:, :, 1::2] << 4)).astype(np.uint8)
+    return codes, scale.reshape(-1)
+
+
 def fill_llama_weights_host(g: LlamaGraph, world: int = 1, rank: int = 0, seed: int = 0):
     """Small configs only (host RNG): full tensors are drawn, then sharded like parallel_opt.py does."""
     for name, (t, shape, kind, shard) in g.weights.items():
@@ -282,6 +321,11 @@ def fill_llama_weights_host(g: LlamaGraph, world: int = 1, rank: int = 0, seed: 
         if kind == "kv_scale":  # the scale the cache helpers quantise with (llama_kv_fp8_values)
             li, which = int(name[1:name.index(".")]), name[name.index(".") + 1]
             t.copyin_numpy(llama_kv_fp8_values(g.cfg, li, which, world, rank)[1])
+            continue
+        if kind == "proj_int4":
+            codes, scale = quantize_w4(llama_weight_values(name, list(shape), "proj", seed), g.cfg.int4_block, g.cfg.dtype)
+            t.copyin_numpy(codes)
+            g.weights[name + ".scale"][0].copyin_numpy(to_storage(scale, g.cfg.dtype))
             continue
         if kind == "proj_fp8":
             codes, scale = quantize_fp8_host(llama_weight_values(name, list(shape), "proj", seed))

@@ -191,6 +191,7 @@ class Node:
     outputs: List[str] = field(default_factory=list)
     name: str = ""
     attrs: Dict[str, Any] = field(default_factory=dict)  # int | float | bytes | list | TensorProto
+    domain: str = ""  # operator set of the node: "" = the default ONNX domain, "com.microsoft" for MatMulNBits
 
     @staticmethod
     def parse(buf) -> "Node":
@@ -203,6 +204,7 @@ class Node:
             elif no == 5:
                 k, val = Node._attr(v)
                 nd.attrs[k] = val
+            elif no == 7: nd.domain = bytes(v).decode()
         return nd
 
     @staticmethod
@@ -240,6 +242,8 @@ class Node:
             elif len(v) and isinstance(v[0], float): a += b"".join(_key(7, 5) + struct.pack("<f", x) for x in v) + _key(20, 0) + _enc_varint(6)
             else: a += _ld(8, b"".join(_enc_varint(int(x)) for x in v)) + _key(20, 0) + _enc_varint(7)
             out += _ld(5, a)
+        if self.domain:  # (default-domain nodes carry no field 7: their bytes are what they always were)
+            out += _ld(7, self.domain.encode())
         return out
 
 
@@ -287,14 +291,23 @@ def load_model(src) -> Model:
         if no == 1: m.ir_version = v
         elif no == 7: m.graph = Graph.parse(v)
         elif no == 8:
-            for n2, _, v2 in _fields(v):
+            fields = list(_fields(v))
+            if any(n2 == 1 and bytes(v2) not in (b"", b"ai.onnx") for n2, _, v2 in fields):
+                continue  # another domain's operator set (com.microsoft): its version does not change the default opset
+            for n2, _, v2 in fields:
                 if n2 == 2: m.opset = v2
     return m
 
 
+MS_DOMAIN = "com.microsoft"
+
+
 def save_model(m: Model) -> bytes:
     opset = _ld(1, b"") + _key(2, 0) + _enc_varint(m.opset)
-    return _key(1, 0) + _enc_varint(m.ir_version) + _ld(2, b"infinitensor_b200") + _ld(7, m.graph.encode()) + _ld(8, opset)
+    out = _key(1, 0) + _enc_varint(m.ir_version) + _ld(2, b"infinitensor_b200") + _ld(7, m.graph.encode()) + _ld(8, opset)
+    if any(nd.domain == MS_DOMAIN for nd in m.graph.nodes):  # the contrib operator set, only when a node uses it
+        out += _ld(8, _ld(1, MS_DOMAIN.encode()) + _key(2, 0) + _enc_varint(1))
+    return out
 
 
 # ------------------------------------------------------------------------------------------------ lowering
@@ -515,6 +528,11 @@ class OnnxStub:
             T[out0] = h.identity(I(0), None)
         elif op == "MatMul":
             T[out0] = h.matmul(I(0), I(1), None, False, False, None, 0)
+        elif op == "MatMulNBits":
+            # com.microsoft MatMulNBits: A, B, scales, [zero_points], [g_idx], [bias]; accuracy_level is read and ignored
+            opt = [I(i) if len(nd.inputs) > i and nd.inputs[i] else None for i in (3, 4, 5)]
+            T[out0] = h.matMulNBits(I(0), I(1), I(2), opt[0], None, a["K"], a["N"], a["block_size"], bits=a.get("bits", 4),
+                                    g_idx=opt[1], bias=opt[2])
         elif op == "Gemm":
             if a.get("alpha", 1.0) != 1.0 or a.get("beta", 1.0) != 1.0:
                 raise NotImplementedError("Gemm: alpha / beta other than 1 are not supported (reference onnx.py:298-300)")
@@ -729,6 +747,16 @@ class OnnxExporter:
         return self._emit("Gemm", [a, b] + ([bias] if bias is not None else []), r,
                           {"transA": int(bool(transA)), "transB": int(bool(transB))})
 
+    def matMulNBits(self, a, b, scales, zero_points, y, K, N, block_size, bits=4, g_idx=None, bias=None):
+        r = self.inner.matMulNBits(a.inner, b.inner, scales.inner, self._in(zero_points), self._in(y), K, N, block_size, bits,
+                                   self._in(g_idx), self._in(bias))
+        ins = [a, b, scales, zero_points, g_idx, bias]
+        while ins[-1] is None:  # trailing absent optional inputs are omitted, inner ones named ""
+            ins.pop()
+        out = self._emit("MatMulNBits", ins, r, {"K": int(K), "N": int(N), "bits": int(bits), "block_size": int(block_size)})
+        self.nodes[-1].domain = MS_DOMAIN
+        return out
+
     def conv(self, x, w, y, ph, pw, sh, sw, dh, dw):
         r = self.inner.conv(x.inner, w.inner, self._in(y), ph, pw, sh, sw, dh, dw)
         return self._emit("Conv", [x, w], r, {"pads": [ph, pw, ph, pw], "strides": [sh, sw], "dilations": [dh, dw],
@@ -910,6 +938,9 @@ def parallel_model(model, world: int, rank: int, new_handler=None) -> Model:
     m = simplify(model, new_handler)
     if world == 1:
         return m
+    for nd in m.graph.nodes:
+        if nd.op_type == "MatMulNBits":
+            raise NotImplementedError(f"MatMulNBits {nd.name}: tensor-parallel sharding of 4-bit weights is not provided")
     shapes = tensor_shapes(m, new_handler)
     g = m.graph
     consts = {t.name: t for t in g.initializers}
