@@ -35,7 +35,8 @@ comes closest.
 
 The kernels deal (head or (KV head, query group), 64-row chunk) units (32 rows for fp32) of the whole batch in equal
 contiguous ranges over min(units, 264) CTAs; `Deal` restates that dealing so failures can be located and so the tests can
-show which dealing states their cases reach.
+show which dealing states their cases reach.  A chunk is 16 KiB of cache: `Deal` and the emulation below also take the head
+width and FP8 caches (one byte per element, tests/kvfp8_64.py), whose chunks hold 16384 / D rows.
 """
 import math
 
@@ -53,8 +54,9 @@ SCALE32 = np.float32(0.08838834764831845)  # the kernels' fp32 1/sqrt(128)
 NAMES = {F32: "fp32", F16: "f16", BF16: "bf16"}
 
 
-def chunk_rows(dt):
-    return 32 if dt == F32 else 64
+def chunk_rows(dt, d=D, kv8=False):
+    """cache rows per 16 KiB chunk: 64 (f16 / bf16) or 32 (fp32) at D = 128, twice that at D = 64; FP8 codes: 16384 / D"""
+    return 16384 // (d * (1 if kv8 else 4 if dt == F32 else 2))
 
 
 # ====================================================================== dealing model
@@ -62,9 +64,9 @@ class Deal:
     """How attn_stream_kernel (grp = 1) and attn_gqa_kernel (grp > 1) deal their units.  A segment is a head (grp = 1) or a
     (KV head, query group) pair; unit u of the batch is (segment, chunk) in row-major order over batch rows."""
 
-    def __init__(self, dt, B, Hq, Hkv, S, pos):
+    def __init__(self, dt, B, Hq, Hkv, S, pos, d=D, kv8=False):
         self.dt, self.B, self.Hq, self.Hkv, self.S = dt, B, Hq, Hkv, S
-        self.CH = chunk_rows(dt)
+        self.CH = chunk_rows(dt, d, kv8)
         self.grp = Hq // Hkv
         if self.grp == 1:
             self.QT, self.GP, self.NQG, self.segs = 1, 1, 1, Hq
@@ -272,11 +274,17 @@ def _exp(x):
         return np.exp(np.asarray(x, np.float64)).astype(np.float32)
 
 
-def _merge(parts, dt, mutation):
+def _out(A, L, dt, vscale):
+    """the output write: A / L rounded to T, or for an FP8 cache fp32(A / L) * v_scale rounded to T"""
+    o = _f(A / L[..., None])
+    return oracle.round_to(o if vscale is None else _f(o * np.float32(vscale)), dt)
+
+
+def _merge(parts, dt, mutation, vscale=None):
     """the last CTA's merge of (m, l, acc) partials in CTA order; also the whole-segment output when there is one partial"""
     if len(parts) == 1:
         m, l, a = parts[0]
-        return oracle.round_to(_f(a / l[..., None]), dt)
+        return _out(a, l, dt, vscale)
     if mutation == "merge_skip_last":
         parts = parts[:-1]
     mw = parts[0][0] if mutation == "merge_slot0_max" else np.max([p[0] for p in parts], axis=0)
@@ -285,7 +293,7 @@ def _merge(parts, dt, mutation):
         cw = np.ones_like(m) if mutation == "merge_ignore_max" else _exp(m - mw)
         L, A = _fma(l, cw, L), _fma(a, cw[..., None], A)
     with np.errstate(invalid="ignore", divide="ignore"):
-        return oracle.round_to(_f(A / L[..., None]), dt)
+        return _out(A, L, dt, vscale)
 
 
 def _stream_dot(qf, k, lpr, epl):
@@ -302,16 +310,18 @@ def _stream_dot(qf, k, lpr, epl):
     return d[..., 0]
 
 
-def emulate_stream_partial(q, K, V, kn, vn, pos, chunks, last, dt, mutation=None):
+def emulate_stream_partial(q, K, V, kn, vn, pos, chunks, last, dt, mutation=None, qs=SCALE32, kv8=False):
     """one CTA's (m, l, acc) of one head in attn_stream_kernel: the consumer warps' per-thread online softmax over `chunks`,
-    the appended row (warp 0, sub-row 0) if `last`, then the sub-row and warp merges.  K, V: the head's rows < pos."""
-    CH = chunk_rows(dt)
-    rpw, lpr = (1, 32) if dt == F32 else (2, 16)
-    epl, U = D // lpr, 4
-    qf = _f(q.astype(np.float32) * SCALE32)
+    the appended row (warp 0, sub-row 0) if `last`, then the sub-row and warp merges.  K, V: the head's rows < pos.
+    FP8 caches (kv8): K, V, kn, vn are the decoded E4M3 values, a lane holds 16 codes of a row, and qs = fp32(k_scale / sqrt(D))."""
+    dw = K.shape[-1]
+    CH = chunk_rows(dt, dw, kv8)
+    lpr = dw // 16 if kv8 else 32 if dt == F32 else dw // 8
+    rpw, epl, U = 32 // lpr, dw // lpr, 4
+    qf = _f(q.astype(np.float32) * np.float32(qs))
     m = np.full((8, rpw), -np.inf, np.float32)
     l = np.zeros((8, rpw), np.float32)
-    acc = np.zeros((8, rpw, D), np.float32)
+    acc = np.zeros((8, rpw, dw), np.float32)
     idx = np.arange(CH).reshape(8, U, rpw)  # chunk row = warp U RPW + uu RPW + sub
     for c in chunks:
         nvalid = pos - c * CH - (1 if mutation == "drop_last_row" and c == chunks[-1] and last else 0)
@@ -338,29 +348,43 @@ def emulate_stream_partial(q, K, V, kn, vn, pos, chunks, last, dt, mutation=None
                 l[0, 0] = _fma(l[0, 0], corr, pn)
                 acc[0, 0] = _fma(pn, vn, _f(acc[0, 0] * corr))
                 m[0, 0] = mx2
-    if rpw == 2:  # sub-row fold (xor 16)
-        mm = m.max(1)
+    o = 1
+    while o < rpw:  # sub-row folds (shuffles xor LPR, 2 LPR, ...): sub-row i takes in sub-row i ^ o
+        x = np.arange(rpw) ^ o
+        m2, l2, a2 = m[:, x], l[:, x], acc[:, x]
+        mm = np.maximum(m, m2)
         live = mm > -np.inf
-        c1 = np.where(live, _exp(m[:, 0] - mm), 0).astype(np.float32)
-        c2 = np.where(live, _exp(m[:, 1] - mm), 0).astype(np.float32)
-        l = _f(_f(l[:, 0] * c1) + _f(l[:, 1] * c2))
-        acc = _f(_f(acc[:, 0] * c1[:, None]) + _f(acc[:, 1] * c2[:, None]))
+        c1 = np.where(live, _exp(m - mm), 0).astype(np.float32)
+        c2 = np.where(live, _exp(m2 - mm), 0).astype(np.float32)
+        l = _f(_f(l * c1) + _f(l2 * c2))
+        acc = _f(_f(acc * c1[..., None]) + _f(a2 * c2[..., None]))
         m = mm
-    else:
-        m, l, acc = m[:, 0], l[:, 0], acc[:, 0]
+        o *= 2
+    m, l, acc = m[:, 0], l[:, 0], acc[:, 0]
     mw = m.max()
     cw = np.where(m > -np.inf, _exp(m - mw), 0).astype(np.float32)
-    L, A = np.float32(0), np.zeros(D, np.float32)
+    L, A = np.float32(0), np.zeros(dw, np.float32)
     for w in range(8):
         L, A = _fma(l[w], cw[w], L), _fma(acc[w], cw[w], A)
     return np.float32(mw), L, A
 
 
-def emulate_gqa_partial(Q, K, V, kn, vn, pos, chunks, last, dt, mutation=None):
-    """one CTA's (m [GP], l [GP], acc [GP, 128]) of one (KV head, query group) segment in attn_gqa_kernel.  Q [GP, 128] with
-    zero padding rows; S = Q K^T per chunk (eight chained k16 MMA steps, or 128 fmaf for fp32), the eight warps' row maxima
-    and sums, P as hi + lo in T (f16 / bf16), O += P V."""
-    CH = chunk_rows(dt)
+def gqa_k_steps(d, kv8=False):
+    """the head-dim columns of each chained k16 MMA step of S = Q K^T: 16 consecutive columns, or for FP8 caches the permuted
+    order (step 4 jj + st: columns 64 jj + 16 qc + 4 st + {0 .. 3} for qc = 0 .. 3)"""
+    if not kv8:
+        return [np.arange(16 * kk, 16 * kk + 16) for kk in range(d // 16)]
+    return [np.array([64 * jj + 16 * qc + 4 * st + e for qc in range(4) for e in range(4)])
+            for jj in range(d // 64) for st in range(4)]
+
+
+def emulate_gqa_partial(Q, K, V, kn, vn, pos, chunks, last, dt, mutation=None, sscale=SCALE32, kv8=False):
+    """one CTA's (m [GP], l [GP], acc [GP, D]) of one (KV head, query group) segment in attn_gqa_kernel.  Q [GP, D] with
+    zero padding rows; S = Q K^T per chunk (D / 16 chained k16 MMA steps, or D fmaf for fp32) times sscale, the eight warps'
+    row maxima and sums, P as hi + lo in T (f16 / bf16), O += P V.  FP8 caches (kv8): K, V, kn, vn are the decoded E4M3
+    values and sscale = fp32(k_scale / sqrt(D))."""
+    D = Q.shape[1]
+    CH = chunk_rows(dt, D, kv8)
     nc = CH // 32
     gp = Q.shape[0]
     Q = Q.astype(np.float32)
@@ -385,9 +409,9 @@ def emulate_gqa_partial(Q, K, V, kn, vn, pos, chunks, last, dt, mutation=None):
                 d = _fma(Q[:, dd, None], kc[None, :, dd], d)
         else:
             d = np.zeros((gp, CH), np.float32)
-            for kk in range(8):
-                d = _f(d + Q[:, 16 * kk:16 * kk + 16].astype(np.float64) @ kc[:, 16 * kk:16 * kk + 16].T.astype(np.float64))
-        s = _f(d * SCALE32)
+            for cols in gqa_k_steps(D, kv8):
+                d = _f(d + Q[:, cols].astype(np.float64) @ kc[:, cols].T.astype(np.float64))
+        s = _f(d * np.float32(sscale))
         s[:, nrows:] = -np.inf
         mnew = np.maximum(m, s.max(1))
         p = _exp(s - mnew[:, None])

@@ -39,9 +39,9 @@ def launch(K, kc, vc, ksc, vsc, q, k, v, pos, dt, flags=0, rope_pos=None):
         flags |= POS_PER_ROW
     pd = K.raw(np.atleast_1d(np.asarray(pos)).astype(np.int64))
     rp = None if rope_pos is None else K.raw(np.asarray(rope_pos, np.int64))
-    out = torch.empty_like(qd)
+    out = torch.full_like(qd, float("nan"))
     wsb = L.lib.it_b200_attention_kvcache_workspace(B, Hq, Smax, D)
-    ws = torch.empty(max(int(wsb), 16), dtype=torch.uint8, device="cuda")
+    ws = torch.full((max(int(wsb), 16),), 0xFF, dtype=torch.uint8, device="cuda")  # NaN in every fp32 slot
     L.check(L.lib.it_b200_attention_kvcache_fp8(dt, K.ptr(kcd), K.ptr(vcd), K.ptr(ksd), K.ptr(vsd), K.ptr(qd), K.ptr(kd), K.ptr(vd),
                                                 K.ptr(pd), 7 | flags, K.ptr(rp), 7, K.ptr(out), B, Hq, Hkv, Smax, D, K.ptr(ws),
                                                 int(wsb), K.stream()))
