@@ -7,13 +7,13 @@ out = (sum_j w_j e4m3(code_v,j)) * scale_v[h], rounded to the activation type on
 
 `quantise` restates the quantiser bit for bit (numpy's float32 division is IEEE, correctly rounded); `attention` is the float64
 reference with a per-element bound, `emulate32` follows the kernels' fp32 order of operations, so that the bound can be shown
-to hold for it and to catch arithmetic slips."""
+to hold for it and to catch arithmetic slips.  The graph oracle (tests/llama_oracle.py) runs `append` and `attention` for
+FP8 caches."""
 import math
 
 import numpy as np
 
 import oracle as O
-from tests.head64_oracle import HeadWidthOracleHandler
 
 F32, F16, BF16 = 1, 10, 16
 E4M3_MAX = 448.0
@@ -171,22 +171,3 @@ def emulate32(kc, vc, ksc, vsc, q, k, v, pos, rows_per_chunk=128, bugs=()):
             out[b, h, 0] = acc / l * f(vsc[hs])
     return out
 
-
-class KvFp8OracleHandler(HeadWidthOracleHandler):
-    """The grouped-query, head-width graph oracle with AttentionKVCache over FP8 caches (uint8 codes + k_scale / v_scale),
-    the rule above; 16-bit caches run the parent's rule."""
-
-    def attentionKVCache(self, kc, vc, q, k, v, pos, y, per_row_positions=False, k_scale=None, v_scale=None):
-        if k_scale is None:
-            return super().attentionKVCache(kc, vc, q, k, v, pos, y, per_row_positions)
-        out = self._out(y, q.dims, q.dt)
-
-        def run():
-            pv = np.asarray(pos.value).ravel()
-            S = kc.dims[2]
-            p = np.clip(pv[:q.dims[0]] if per_row_positions else np.full(q.dims[0], int(pv[0])), 0, S - 1)
-            append(kc.value, vc.value, np.asarray(k.value, np.float32), np.asarray(v.value, np.float32), k_scale.value,
-                   v_scale.value, p)
-            ref, _ = attention(kc.value, vc.value, k_scale.value, v_scale.value, q.value, p, q.dt)
-            return O.round_to(ref.astype(np.float32), q.dt)
-        return self._rec(run, [kc, vc, q, k, v, pos, k_scale, v_scale], [out])

@@ -1,60 +1,11 @@
 """smoke(): one tiny Llama-shape decode step on cuda:0 through the public graph API, CUDA-graph replayed,
 checked against the CPU oracle executing the same graph description."""
-import numpy as np
-
-
-def run_llama_parity(dtype=16, layers=2, batch=4, pos=5, steps=2, cudagraph=True, cfg=None, tol=None):
-    from infinitensor_b200 import backend as B
-    from infinitensor_b200 import graphs as G
-    from oracle.graph_oracle import OracleHandler
-
-    cfg = cfg or G.LlamaConfig.tiny(dtype=dtype, layers=layers, batch=batch)
-    rt = B.CudaRuntime(0)
-    h = B.GraphHandler(rt)
-    g = G.build_llama_decode(h, cfg)
-    h.data_malloc()
-    G.fill_llama_weights_host(g)
-    oh = OracleHandler()
-    og = G.build_llama_decode(oh, cfg)
-    G.fill_llama_weights_host(og)
-    for li in range(cfg.layers):
-        for which, (ct, oct_) in (("k", (g.k_caches[li], og.k_caches[li])), ("v", (g.v_caches[li], og.v_caches[li]))):
-            vals = G.to_storage(G.llama_cache_values(cfg, li, which), cfg.dtype)
-            ct.copyin_numpy(vals)
-            oct_.copyin_numpy(vals)
-    rng = np.random.default_rng(1)
-    worst = 0.0
-    for step in range(steps):
-        ids = rng.integers(0, cfg.vocab, size=(cfg.batch, 1)).astype(np.int64)
-        p = np.full((cfg.batch, 1), pos + step, np.int64)
-        for hh, gg in ((h, g), (oh, og)):
-            gg.input_ids.copyin_numpy(ids)
-            gg.position_ids.copyin_numpy(p)
-        if cudagraph:
-            h.run_with_cudagraph()
-        else:
-            h.run()
-        oh.run()
-        got = G.from_storage(g.logits.copyout_numpy(), cfg.dtype).astype(np.float64)
-        ref = og.logits.f32().astype(np.float64)
-        # end-to-end criterion of the reference: rtol = atol = 1e-3 else argmax-equal
-        # (examples/python/llama_kvcache_inference.py:133-141); 16-bit storage gets its rounding step
-        t = tol or {1: 1e-3, 10: 4e-3, 16: 3e-2}[cfg.dtype]
-        err = np.abs(got - ref).max() / max(np.abs(ref).max(), 1e-6)
-        worst = max(worst, err)
-        assert err < t, f"step {step}: logits rel-to-max error {err:.3e} >= {t}"
-        # the appended KV rows (rotated k of this step): the storage type's rounding step -- the RoPE arithmetic runs on the
-        # GPU's cosf / sinf (tolerance, not bit-equality; the cache rows that are NOT appended are checked bit-exact in
-        # tests/test_gpu_kernels.py::test_attention_parity)
-        k_got = G.from_storage(g.k_caches[0].copyout_numpy(), cfg.dtype)
-        assert np.allclose(k_got[:, :, pos + step], og.k_caches[0].f32()[:, :, pos + step], rtol=t, atol=t)
-    if cudagraph:
-        assert rt.cuda_graph_capture_count() == 1, "graph must be captured once and replayed"
-    return worst, rt.kernel_launches()
 
 
 def run():
-    worst, launches = run_llama_parity()
+    from infinitensor_b200 import graphs as G
+    from tests.llama_oracle import run_llama_parity
+    worst, launches, _ = run_llama_parity(G.LlamaConfig.tiny(dtype=16, layers=2, batch=4), pos=5, steps=2)
     assert launches > 0
     print(f"smoke ok: tiny Llama decode (bf16, 2 layers, CUDA graph replay) max rel err {worst:.3e}, "
           f"{launches} kernel launches")

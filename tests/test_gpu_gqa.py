@@ -1,5 +1,5 @@
 """Grouped-query decode attention on the GPU: it_b200_attention_kvcache_gqa against the oracle's AttentionKVCache run
-per group member (tests/gqa_oracle.py), and whole GQA Llama graphs against the graph oracle with that rule."""
+per group member (tests/llama_oracle.py), and whole GQA Llama graphs against the graph oracle with that rule."""
 import os
 import subprocess
 import sys
@@ -10,7 +10,7 @@ import pytest
 pytestmark = pytest.mark.gpu
 
 import oracle
-from tests.gqa_oracle import GqaOracleHandler, attention_kvcache_gqa, run_gqa_llama_parity
+from tests.llama_oracle import attention_kvcache_gqa, oracle_graph, run_llama_parity
 
 F32, F16, BF16 = 1, 10, 16
 TOL = {F32: 1e-5, F16: 1e-3, BF16: 1e-2}  # as test_attention_parity (SURVEY 8(c))
@@ -156,10 +156,9 @@ def _gqa_cfg(dtype, kv_heads, layers=2, d=512, heads=4, batch=16, s_max=64, ffn=
 @pytest.mark.parametrize("kv_heads", [2, 1])
 @pytest.mark.parametrize("fused", [True, False])
 @pytest.mark.parametrize("cudagraph", [True, False])
-def test_gqa_llama_graph_parity(dtype, kv_heads, fused, cudagraph, monkeypatch):
-    if not fused:
-        monkeypatch.setenv("ITB_NO_FUSION", "1")
-    _, sched = run_gqa_llama_parity(_gqa_cfg(dtype, kv_heads), pos=5, steps=2, cudagraph=cudagraph)
+def test_gqa_llama_graph_parity(dtype, kv_heads, fused, cudagraph):
+    env = None if fused else {"ITB_NO_FUSION": "1"}
+    _, _, sched = run_llama_parity(_gqa_cfg(dtype, kv_heads), pos=5, steps=2, cudagraph=cudagraph, env=env)
     if fused:
         assert sum(s.startswith("AttentionRope") for s in sched) == 2
 
@@ -170,7 +169,7 @@ def test_gqa_llama3_width_graph_parity():
     full = G.LlamaConfig.llama3_8b()
     cfg = G.LlamaConfig(layers=2, d_model=full.d_model, heads=full.heads, kv_heads=full.kv_heads, head_dim=128, ffn=full.ffn,
                         vocab=2048, s_max=1024, batch=16, dtype=BF16)
-    run_gqa_llama_parity(cfg, pos=511, steps=1)
+    run_llama_parity(cfg, pos=511, steps=1)
 
 
 def _ngpu():
@@ -190,12 +189,7 @@ def test_gqa_tensor_parallel_two_gpus(tmp_path):
     subprocess.run(cmd, check=True, env=env, cwd=ROOT, timeout=600)
     cfg = G.LlamaConfig(layers=2, d_model=1024, heads=8, kv_heads=2, head_dim=128, ffn=2816, vocab=2048, s_max=64, batch=16,
                         dtype=BF16)
-    oh = GqaOracleHandler()
-    g = G.build_llama_decode(oh, cfg)
-    G.fill_llama_weights_host(g)
-    for li in range(cfg.layers):
-        g.k_caches[li].copyin_numpy(G.to_storage(G.llama_cache_values(cfg, li, "k"), BF16))
-        g.v_caches[li].copyin_numpy(G.to_storage(G.llama_cache_values(cfg, li, "v"), BF16))
+    oh, g = oracle_graph(cfg)
     refs = []
     for step in range(3):
         g.input_ids.copyin_numpy((np.arange(cfg.batch, dtype=np.int64).reshape(-1, 1) * 7 + step) % cfg.vocab)

@@ -12,17 +12,18 @@ F32, F16, BF16 = 1, 10, 16
 @pytest.mark.parametrize("dtype", [F32, F16, BF16])
 @pytest.mark.parametrize("cudagraph", [False, True])
 def test_llama_decode_parity(dtype, cudagraph):
-    from tests.smoke_impl import run_llama_parity
-    worst, launches = run_llama_parity(dtype=dtype, layers=2, batch=4, pos=5, steps=3, cudagraph=cudagraph)
+    from infinitensor_b200 import graphs as G
+    from tests.llama_oracle import run_llama_parity
+    _, launches, _ = run_llama_parity(G.LlamaConfig.tiny(dtype=dtype, layers=2, batch=4), pos=5, steps=3, cudagraph=cudagraph)
     assert launches > 0
 
 
 def test_llama_decode_batch16_wide():
     """d=1024 / ffn=2816 / B=16: the skinny TMA GEMM path (M=16) inside the graph."""
     from infinitensor_b200 import graphs as G
-    from tests.smoke_impl import run_llama_parity
+    from tests.llama_oracle import run_llama_parity
     cfg = G.LlamaConfig(layers=2, d_model=1024, heads=8, head_dim=128, ffn=2816, vocab=2048, s_max=128, batch=16, dtype=BF16)
-    run_llama_parity(cfg=cfg, pos=77, steps=2)
+    run_llama_parity(cfg, pos=77, steps=2)
 
 
 def test_llama_decode_baseline_width():
@@ -31,9 +32,9 @@ def test_llama_decode_baseline_width():
     and gate/up, o, down, the 32000-wide logits), the 512-head streaming attention with folded RoPE, the fused schedule and
     CUDA-graph replay, end to end against the oracle."""
     from infinitensor_b200 import graphs as G
-    from tests.smoke_impl import run_llama_parity
+    from tests.llama_oracle import run_llama_parity
     cfg = G.LlamaConfig(layers=2, d_model=4096, heads=32, head_dim=128, ffn=11008, vocab=32000, s_max=1024, batch=16, dtype=BF16)
-    run_llama_parity(cfg=cfg, pos=511, steps=1)
+    run_llama_parity(cfg, pos=511, steps=1)
 
 
 @pytest.mark.parametrize("dtype", [BF16, F16])
@@ -42,14 +43,14 @@ def test_llama_decode_fp8_weights(dtype):
     with FP8 E4M3 weight codes + per-column scales dequantised inside the GEMM; the oracle executes the same graph with the
     dequantised weights in fp32.  CUDA-graph replay, two steps."""
     from infinitensor_b200 import backend as B, graphs as G
-    from tests.smoke_impl import run_llama_parity
+    from tests.llama_oracle import run_llama_parity
     cfg = G.LlamaConfig(layers=2, d_model=1024, heads=8, head_dim=128, ffn=2816, vocab=2048, s_max=128, batch=16, dtype=dtype,
                         fp8_weights=True)
     h = B.GraphHandler(B.CudaRuntime(0))
     G.build_llama_decode(h, cfg)
     sc = h.schedule()
     assert sc.count("MatMulGroup:MatMul+MatMul+MatMul") == 2 and sc.count("MatMulAdd:MatMul+Add") == 4
-    run_llama_parity(cfg=cfg, pos=77, steps=2)
+    run_llama_parity(cfg, pos=77, steps=2)
 
 
 def test_matmul_512_config1():

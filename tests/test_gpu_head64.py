@@ -10,7 +10,7 @@ pytestmark = pytest.mark.gpu
 
 import oracle
 from tests import attn64
-from tests.head64_oracle import HeadWidthOracleHandler, attention_kvcache_d
+from tests.llama_oracle import attention_kvcache_d, run_llama_parity
 
 F32, F16, BF16 = 1, 10, 16
 D = 64
@@ -260,57 +260,18 @@ def test_head64_attention_float64_bound(K, case, dt):
 
 
 # ====================================================================== graphs
-def _fill_caches(cfg, g, og, G):
-    for li in range(cfg.layers):
-        for which, ct, oct_ in (("k", g.k_caches[li], og.k_caches[li]), ("v", g.v_caches[li], og.v_caches[li])):
-            vals = G.to_storage(G.llama_cache_values(cfg, li, which), cfg.dtype)
-            ct.copyin_numpy(vals)
-            oct_.copyin_numpy(vals)
-
-
 @pytest.mark.parametrize("dtype", [BF16, F16])
 @pytest.mark.parametrize("mode", ["fused_cudagraph", "fused", "unfused"])
-def test_tinyllama_graph_parity(dtype, mode, monkeypatch):
+def test_tinyllama_graph_parity(dtype, mode):
     """two TinyLlama-width layers (32 query heads of 64 over 4 KV heads, ffn 5632) at B 16 against the oracle, positions
     127 and 128 (the second crosses the 128-row chunk boundary)"""
-    from infinitensor_b200 import backend as B, graphs as G
-    if mode == "unfused":
-        monkeypatch.setenv("ITB_NO_FUSION", "1")
+    from infinitensor_b200 import graphs as G
     cfg = G.LlamaConfig.tinyllama_1b(batch=16, s_max=256, dtype=dtype, layers=2)
     cfg.vocab = 2048
-    rt = B.CudaRuntime(0)
-    h = B.GraphHandler(rt)
-    g = G.build_llama_decode(h, cfg)
-    h.data_malloc()
-    G.fill_llama_weights_host(g)
-    oh = HeadWidthOracleHandler()
-    og = G.build_llama_decode(oh, cfg)
-    G.fill_llama_weights_host(og)
-    _fill_caches(cfg, g, og, G)
-    sched = h.schedule()
+    env = {"ITB_NO_FUSION": "1"} if mode == "unfused" else None
+    _, _, sched = run_llama_parity(cfg, pos=127, steps=2, cudagraph=mode == "fused_cudagraph", env=env)
     if mode != "unfused":
         assert sum(s.startswith("AttentionRope") for s in sched) == cfg.layers
-    rng = np.random.default_rng(1)
-    tol = {F16: 4e-3, BF16: 3e-2}[dtype]
-    for step, pos in enumerate((127, 128)):
-        ids = rng.integers(0, cfg.vocab, size=(cfg.batch, 1)).astype(np.int64)
-        p = np.full((cfg.batch, 1), pos, np.int64)
-        for gg in (g, og):
-            gg.input_ids.copyin_numpy(ids)
-            gg.position_ids.copyin_numpy(p)
-        if mode == "fused_cudagraph":
-            h.run_with_cudagraph()
-        else:
-            h.run()
-        oh.run()
-        got = G.from_storage(g.logits.copyout_numpy(), dtype).astype(np.float64)
-        ref = og.logits.f32().astype(np.float64)
-        err = np.abs(got - ref).max() / max(np.abs(ref).max(), 1e-6)
-        assert err < tol, f"step {step}: logits rel-to-max error {err:.3e}"
-        k_got = G.from_storage(g.k_caches[0].copyout_numpy(), dtype)
-        assert np.allclose(k_got[:, :, pos], og.k_caches[0].f32()[:, :, pos], rtol=tol, atol=tol)
-    if mode == "fused_cudagraph":
-        assert rt.cuda_graph_capture_count() == 1
 
 
 def test_gpt2_decode_matches_forward():

@@ -1,6 +1,7 @@
 """Decode attention over an FP8 E4M3 KV cache on the GPU: it_b200_attention_kvcache_fp8 against the float64 oracle of
 tests/kvfp8_oracle.py (per element, with its bound), the appended codes bit for bit, RoPE folded against RoPE + the unfused
-launcher, and whole Llama graphs with LlamaConfig(kv_fp8=True) against the graph oracle with the same rule."""
+launcher, and whole Llama graphs with LlamaConfig(kv_fp8=True) against the graph oracle with the same rule
+(tests/llama_oracle.py)."""
 import numpy as np
 import pytest
 
@@ -8,6 +9,7 @@ pytestmark = pytest.mark.gpu
 
 import oracle
 from tests import kvfp8_oracle as KV
+from tests.llama_oracle import run_llama_parity
 
 F16, BF16 = 10, 16
 NAN = np.uint8(0x7F)
@@ -159,55 +161,11 @@ def test_fp8_refusals(K):
 
 
 # ---------------------------------------------------------------------------------------------------- whole graphs
-def run_graph(cfg, pos=5, steps=3, cudagraph=True, fused=True, tol=3e-2):
-    """The device graph with FP8 caches vs KvFp8OracleHandler: logits rel-to-max error per step, and the appended codes of
-    layer 0 bit for bit.  fused=False disables the RoPE -> attention fold (ITB_FUSION_MASK without bit 5)."""
-    import os
-    from infinitensor_b200 import backend as B
-    from infinitensor_b200 import graphs as G
-    old = os.environ.get("ITB_FUSION_MASK")
-    if not fused:
-        os.environ["ITB_FUSION_MASK"] = str((127 | 256 | 512 | 1024 | 2048) & ~32)
-    try:
-        rt = B.CudaRuntime(0)
-        h = B.GraphHandler(rt)
-        g = G.build_llama_decode(h, cfg)
-        h.data_malloc()
-        sched = h.schedule()
-    finally:
-        if old is None:
-            os.environ.pop("ITB_FUSION_MASK", None)
-        else:
-            os.environ["ITB_FUSION_MASK"] = old
-    G.fill_llama_weights_host(g)
-    oh = KV.KvFp8OracleHandler()
-    og = G.build_llama_decode(oh, cfg)
-    G.fill_llama_weights_host(og)
-    for li in range(cfg.layers):
-        for which, ct, oct_ in (("k", g.k_caches[li], og.k_caches[li]), ("v", g.v_caches[li], og.v_caches[li])):
-            codes, _ = G.llama_kv_fp8_values(cfg, li, which)
-            ct.copyin_numpy(codes)
-            oct_.copyin_numpy(codes)
-    rng = np.random.default_rng(1)
-    for step in range(steps):
-        ids = rng.integers(0, cfg.vocab, size=(cfg.batch, 1)).astype(np.int64)
-        p = np.full((cfg.batch, 1), pos + step, np.int64)
-        for gg in (g, og):
-            gg.input_ids.copyin_numpy(ids)
-            gg.position_ids.copyin_numpy(p)
-        h.run_with_cudagraph() if cudagraph else h.run()
-        oh.run()
-        got = G.from_storage(g.logits.copyout_numpy(), cfg.dtype).astype(np.float64)
-        ref = og.logits.f32().astype(np.float64)
-        err = np.abs(got - ref).max() / max(np.abs(ref).max(), 1e-6)
-        assert err < tol, f"step {step}: logits rel-to-max error {err:.3e} >= {tol}"
-        kg = g.k_caches[0].copyout_numpy()[:, :, pos + step]
-        ko = og.k_caches[0].copyout_numpy()[:, :, pos + step]
-        # the appended codes come from activations that already differ in their last bits: allow a code step on a few
-        assert np.mean(kg != ko) < 0.05, "appended k codes of layer 0 differ from the oracle's beyond rounding"
-    if cudagraph:
-        assert rt.cuda_graph_capture_count() == 1
-    return sched
+def run_graph(cfg, pos=5, steps=3, cudagraph=True, fused=True):
+    """The device graph with FP8 caches against the graph oracle (tests/llama_oracle.py); fused=False disables the
+    RoPE -> attention fold (ITB_FUSION_MASK without bit 5).  Returns the schedule."""
+    env = None if fused else {"ITB_FUSION_MASK": str((127 | 256 | 512 | 1024 | 2048) & ~32)}
+    return run_llama_parity(cfg, pos, steps, cudagraph, env=env, tol=3e-2)[2]
 
 
 @pytest.mark.parametrize("cudagraph", [False, True])

@@ -188,82 +188,39 @@ def _argmax_agree(got, ref, tol):
 
 def run_prompt_then_decode(cfg, S, p0, decode_steps, cudagraph, tol):
     """prompt step of S tokens at p0 .. p0 + S - 1 (per-row [B, S] positions), then decode steps, on the device and on the
-    oracle; every step's logits against the oracle's (rel-to-max error < tol, argmax agreement)"""
+    oracle (tests/llama_oracle.py); every step's logits against the oracle's (rel-to-max error < tol, argmax agreement)"""
     from infinitensor_b200 import backend as B_, graphs as G
-    from tests.prompt_oracle import PromptOracleHandler
+    from tests import llama_oracle as L
     rt = B_.CudaRuntime(0)
     rng = np.random.default_rng(3)
     Bn = cfg.batch
     caches = [G.to_storage(rng.standard_normal((Bn, cfg.n_kv, cfg.s_max, cfg.head_dim)).astype(np.float32) * 0.5, cfg.dtype)
               for _ in range(2 * cfg.layers)]
 
-    def pair(seq):
-        h = B_.GraphHandler(rt)
-        g = G.build_llama_decode(h, cfg, seq=seq)
-        h.data_malloc()
-        G.fill_llama_weights_host(g)
-        oh = PromptOracleHandler()
-        og = G.build_llama_decode(oh, cfg, seq=seq)
-        G.fill_llama_weights_host(og)
-        return (h, g), (oh, og)
-
-    def step(dev, orc, ids, pos, cache_vals):
-        (h, g), (oh, og) = dev, orc
-        for gg in (g, og):
-            for t, c in zip(gg.k_caches + gg.v_caches, cache_vals):
-                t.copyin_numpy(c)
-            gg.input_ids.copyin_numpy(ids)
-            gg.position_ids.copyin_numpy(pos)
-        if cudagraph:
-            h.run_with_cudagraph()
-        else:
-            h.run()
-        oh.run()
-        got = G.from_storage(g.logits.copyout_numpy(), cfg.dtype).astype(np.float64)
-        ref = og.logits.f32().astype(np.float64)
-        err = np.abs(got - ref).max() / max(np.abs(ref).max(), 1e-6)
-        assert err < tol, f"logits rel-to-max error {err:.3e} >= {tol}"
+    def step(p, ids, pos, what):
+        got, ref = L.llama_step(p, ids, pos, cudagraph)
+        err = L.rel_err(got, ref)
+        assert np.isfinite(got).all(), f"{what}: non-finite logits"
+        assert err < tol, f"{what}: logits rel-to-max error {err:.3e} >= {tol}"
         assert _argmax_agree(got, ref, tol)
-        dev_caches = [t.copyout_numpy() for t in g.k_caches + g.v_caches]
-        orc_caches = [G.to_storage(t.f32(), cfg.dtype) for t in og.k_caches + og.v_caches]
-        return err, dev_caches, orc_caches
+        return err
 
-    dev, orc = pair(S)
+    prompt = L.llama_pair(cfg, seq=S, caches=caches, rt=rt)
     ids = rng.integers(0, cfg.vocab, size=(Bn, S)).astype(np.int64)
-    pos = np.broadcast_to(p0 + np.arange(S), (Bn, S)).astype(np.int64).copy()
-    worst, dcache, ocache = step(dev, orc, ids, pos, caches)
+    worst = step(prompt, ids, np.broadcast_to(p0 + np.arange(S), (Bn, S)).astype(np.int64).copy(), "prompt step")
     # the appended k rows of layer 0 agree with the oracle's (the projections differ by rounding only)
-    kd, ko = G.from_storage(dcache[0], cfg.dtype), G.from_storage(ocache[0], cfg.dtype)
-    assert np.allclose(kd[:, :, p0:p0 + S], ko[:, :, p0:p0 + S], rtol=tol, atol=tol)
-    assert np.array_equal(dcache[0][:, :, :p0], caches[0][:, :, :p0])
+    L.check_appended_k(prompt, slice(p0, p0 + S), tol)
+    assert np.array_equal(prompt.g.k_caches[0].copyout_numpy()[:, :, :p0], caches[0][:, :, :p0])
     if decode_steps:
-        dev1, orc1 = pair(1)
+        # each side continues from its own caches
+        dec = L.llama_pair(cfg, caches=L.cache_values(prompt.g), oracle_caches=L.cache_values(prompt.og), rt=rt)
         for i in range(decode_steps):
             ids = rng.integers(0, cfg.vocab, size=(Bn, 1)).astype(np.int64)
-            pos = np.full((Bn, 1), p0 + S + i, np.int64)
-            # each side continues from its own caches
-            (h, g), (oh, og) = dev1, orc1
-            for t, c in zip(g.k_caches + g.v_caches, dcache):
-                t.copyin_numpy(c)
-            for t, c in zip(og.k_caches + og.v_caches, ocache):
-                t.copyin_numpy(c)
-            for gg in (g, og):
-                gg.input_ids.copyin_numpy(ids)
-                gg.position_ids.copyin_numpy(pos)
-            h.run_with_cudagraph() if cudagraph else h.run()
-            oh.run()
-            got = G.from_storage(g.logits.copyout_numpy(), cfg.dtype).astype(np.float64)
-            ref = og.logits.f32().astype(np.float64)
-            err = np.abs(got - ref).max() / max(np.abs(ref).max(), 1e-6)
-            assert err < tol, f"decode step {i}: logits rel-to-max error {err:.3e} >= {tol}"
-            assert _argmax_agree(got, ref, tol)
-            worst = max(worst, err)
-            dcache = [t.copyout_numpy() for t in g.k_caches + g.v_caches]
-            ocache = [G.to_storage(t.f32(), cfg.dtype) for t in og.k_caches + og.v_caches]
-    return worst, dev[0].schedule()
+            worst = max(worst, step(dec, ids, np.full((Bn, 1), p0 + S + i, np.int64), f"decode step {i}"))
+    return worst, prompt.schedule
 
 
-BF16_TOL = 3e-2  # the bf16 graph tolerance of the decode parity tests (tests/gqa_oracle.py)
+BF16_TOL = 3e-2  # the bf16 graph tolerance of the decode parity tests (tests/llama_oracle.py)
 
 
 @pytest.mark.parametrize("cudagraph", [False, True])

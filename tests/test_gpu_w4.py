@@ -1,12 +1,13 @@
 """4-bit MatMulNBits on the GPU: it_b200_matmul_nbits against the float64 oracle of tests/w4_oracle.py (per element, with its
 bound), in NaN-poisoned guarded outputs and run twice bit for bit; the kernel's name in a profile; and int4 Llama graphs against
-the graph oracle."""
+the graph oracle (tests/llama_oracle.py)."""
 import numpy as np
 import pytest
 
 pytestmark = pytest.mark.gpu
 
 import oracle
+from tests import llama_oracle as L
 from tests import ref64
 from tests import w4_oracle as W
 
@@ -175,52 +176,10 @@ def test_w4_kernel_names_in_profile(K):
 
 
 # ---------------------------------------------------------------------------------------------------- whole graphs
-def run_graph(cfg, pos=5, steps=3, cudagraph=True, fused=True, prompt=0, tol=3e-2, handler=None):
-    """The device graph with int4 weights vs W4OracleHandler: logits rel-to-max error per step.  prompt > 0: a prompt step of that
-    many tokens first (seq = prompt), then `steps` decode steps on a second graph sharing the caches' contents."""
-    import os
-    from infinitensor_b200 import backend as B
-    from infinitensor_b200 import graphs as G
-    old = os.environ.get("ITB_FUSION_MASK")
-    if not fused:
-        os.environ["ITB_FUSION_MASK"] = "0"
-    try:
-        rt = B.CudaRuntime(0)
-        h = B.GraphHandler(rt)
-        g = G.build_llama_decode(h, cfg)
-        h.data_malloc()
-        sched = h.schedule()
-    finally:
-        if old is None:
-            os.environ.pop("ITB_FUSION_MASK", None)
-        else:
-            os.environ["ITB_FUSION_MASK"] = old
-    G.fill_llama_weights_host(g)
-    oh = W.W4OracleHandler()
-    og = G.build_llama_decode(oh, cfg)
-    G.fill_llama_weights_host(og)
-    for li in range(cfg.layers):
-        for which, ct, oct_ in (("k", g.k_caches[li], og.k_caches[li]), ("v", g.v_caches[li], og.v_caches[li])):
-            v = G.to_storage(G.llama_cache_values(cfg, li, which), cfg.dtype)
-            ct.copyin_numpy(v)
-            oct_.copyin_numpy(v)
-    rng = np.random.default_rng(1)
-    for step in range(steps):
-        ids = rng.integers(0, cfg.vocab, size=(cfg.batch, 1)).astype(np.int64)
-        p = np.full((cfg.batch, 1), pos + step, np.int64)
-        for gg in (g, og):
-            gg.input_ids.copyin_numpy(ids)
-            gg.position_ids.copyin_numpy(p)
-        h.run_with_cudagraph() if cudagraph else h.run()
-        oh.run()
-        got = G.from_storage(g.logits.copyout_numpy(), cfg.dtype).astype(np.float64)
-        ref = og.logits.f32().astype(np.float64)
-        assert np.isfinite(got).all()
-        err = np.abs(got - ref).max() / max(np.abs(ref).max(), 1e-6)
-        assert err < tol, f"step {step}: logits rel-to-max error {err:.3e} >= {tol}"
-    if cudagraph:
-        assert rt.cuda_graph_capture_count() == 1
-    return sched
+def run_graph(cfg, pos=5, steps=3, cudagraph=True, fused=True):
+    """The device graph with int4 weights against the graph oracle (tests/llama_oracle.py); fused=False plans the unfused
+    schedule (ITB_FUSION_MASK=0).  Returns the schedule."""
+    return L.run_llama_parity(cfg, pos, steps, cudagraph, env=None if fused else {"ITB_FUSION_MASK": "0"}, tol=3e-2)[2]
 
 
 @pytest.mark.parametrize("cudagraph", [False, True])
@@ -247,6 +206,20 @@ def test_w4_llama7b_width_two_layers(K):
     run_graph(cfg, pos=200, steps=2)
 
 
+@pytest.mark.parametrize("cudagraph", [False, True])
+@pytest.mark.parametrize("shape", ["tiny", "tinyllama_width"])
+def test_w4_llama_kv_fp8(K, shape, cudagraph):
+    """int4 weights with an FP8 KV cache"""
+    from infinitensor_b200 import graphs as G
+    if shape == "tiny":
+        cfg = G.LlamaConfig.tiny(kv_fp8=True)
+        cfg.int4_block, cfg.vocab = 32, 1024
+        run_graph(cfg, cudagraph=cudagraph)
+    else:
+        run_graph(G.LlamaConfig.tinyllama_1b(batch=4, s_max=512, layers=2, kv_fp8=True, int4_block=64), pos=300,
+                  cudagraph=cudagraph)
+
+
 @pytest.mark.parametrize("dt", [F16, BF16])
 def test_w4_prompt_then_decode(K, dt):
     """a 40-token prompt step (dequantise path: 4 x 40 rows) fills the caches, then decode steps continue from them"""
@@ -254,51 +227,22 @@ def test_w4_prompt_then_decode(K, dt):
     from infinitensor_b200 import graphs as G
     cfg = G.LlamaConfig.tiny(dtype=dt, batch=4)
     cfg.int4_block, cfg.vocab = 64, 1024
-    S = 40
+    S, tol = 40, 3e-2
     rt = B.CudaRuntime(0)
-    hp, hd = B.GraphHandler(rt), B.GraphHandler(rt)
-    gp, gd = G.build_llama_decode(hp, cfg, seq=S), G.build_llama_decode(hd, cfg)
-    hp.data_malloc()
-    hd.data_malloc()
-    oh = W.W4OracleHandler()
-    op_, od = G.build_llama_decode(oh, cfg, seq=S), None
-    for gg in (gp, gd, op_):
-        G.fill_llama_weights_host(gg)
-    zeros = np.zeros((cfg.batch, cfg.n_kv, cfg.s_max, cfg.head_dim), np.float32)
-    for li in range(cfg.layers):
-        for c in (gp.k_caches[li], gp.v_caches[li], op_.k_caches[li], op_.v_caches[li]):
-            c.copyin_numpy(G.to_storage(zeros, dt))
+    zeros = G.to_storage(np.zeros((cfg.batch, cfg.n_kv, cfg.s_max, cfg.head_dim), np.float32), dt)
+    p = L.llama_pair(cfg, seq=S, caches=[zeros] * (2 * cfg.layers), rt=rt)
     rng = np.random.default_rng(4)
     ids = rng.integers(0, cfg.vocab, size=(cfg.batch, S)).astype(np.int64)
-    pos = np.tile(np.arange(S, dtype=np.int64), (cfg.batch, 1))
-    for gg in (gp, op_):
-        gg.input_ids.copyin_numpy(ids)
-        gg.position_ids.copyin_numpy(pos)
-    hp.run()
-    oh.run()
-    got = G.from_storage(gp.logits.copyout_numpy(), dt).astype(np.float64)
-    ref = op_.logits.f32().astype(np.float64)
-    assert np.abs(got - ref).max() / np.abs(ref).max() < 3e-2
-    # decode steps from the prompt's caches, on the device graph and on a decode oracle graph holding the oracle's caches
-    oh2 = W.W4OracleHandler()
-    od = G.build_llama_decode(oh2, cfg)
-    G.fill_llama_weights_host(od)
-    for li in range(cfg.layers):
-        gd.k_caches[li].copyin_numpy(gp.k_caches[li].copyout_numpy())
-        gd.v_caches[li].copyin_numpy(gp.v_caches[li].copyout_numpy())
-        od.k_caches[li].copyin_numpy(op_.k_caches[li].copyout_numpy())
-        od.v_caches[li].copyin_numpy(op_.v_caches[li].copyout_numpy())
+    got, ref = L.llama_step(p, ids, np.tile(np.arange(S, dtype=np.int64), (cfg.batch, 1)), cudagraph=False)
+    assert np.isfinite(got).all() and L.rel_err(got, ref) < tol
+    L.check_appended_k(p, slice(0, S), tol)
+    # decode steps from the prompt's caches: each side continues from its own
+    d = L.llama_pair(cfg, caches=L.cache_values(p.g), oracle_caches=L.cache_values(p.og), rt=rt)
     for step in range(3):
         ids1 = rng.integers(0, cfg.vocab, size=(cfg.batch, 1)).astype(np.int64)
-        p1 = np.full((cfg.batch, 1), S + step, np.int64)
-        for gg in (gd, od):
-            gg.input_ids.copyin_numpy(ids1)
-            gg.position_ids.copyin_numpy(p1)
-        hd.run_with_cudagraph()
-        oh2.run()
-        got = G.from_storage(gd.logits.copyout_numpy(), dt).astype(np.float64)
-        ref = od.logits.f32().astype(np.float64)
-        assert np.abs(got - ref).max() / np.abs(ref).max() < 3e-2, f"decode step {step}"
+        got, ref = L.llama_step(d, ids1, np.full((cfg.batch, 1), S + step, np.int64))
+        assert np.isfinite(got).all() and L.rel_err(got, ref) < tol, f"decode step {step}"
+        L.check_appended_k(d, S + step, tol)
 
 
 def test_w4_onnx_import(K):
@@ -311,24 +255,17 @@ def test_w4_onnx_import(K):
     exp = X.OnnxExporter(B.GraphHandler(B.HostPlanRuntime()))
     ge = G.build_llama_decode(exp, cfg)
     G.fill_llama_weights_host(ge)
-    rt = B.CudaRuntime(0)
-    stub = X.OnnxStub(exp.save(), handler=B.GraphHandler(rt))
-    oh = W.W4OracleHandler()
-    og = G.build_llama_decode(oh, cfg)
-    G.fill_llama_weights_host(og)
+    stub = X.OnnxStub(exp.save(), handler=B.GraphHandler(B.CudaRuntime(0)))
+    oh, og = L.oracle_graph(cfg)
     rng = np.random.default_rng(3)
     feeds = {ge.input_ids.name: rng.integers(0, cfg.vocab, size=(cfg.batch, 1)).astype(np.int64),
              ge.position_ids.name: np.full((cfg.batch, 1), 7, np.int64)}
     og.input_ids.copyin_numpy(feeds[ge.input_ids.name])
     og.position_ids.copyin_numpy(feeds[ge.position_ids.name])
-    for li in range(cfg.layers):
-        for which, ce, co in (("k", ge.k_caches[li], og.k_caches[li]), ("v", ge.v_caches[li], og.v_caches[li])):
-            feeds[ce.name] = G.to_storage(G.llama_cache_values(cfg, li, which), cfg.dtype)
-            co.copyin_numpy(feeds[ce.name])
+    feeds.update((t.name, c) for t, c in zip(ge.k_caches + ge.v_caches, L.llama_caches(cfg)))
     for name, arr in feeds.items():
         stub.inputs[name].copyin_numpy(arr)
     stub.run()
     oh.run()
     got = G.from_storage(stub.outputs[ge.logits.name].copyout_numpy(), cfg.dtype).astype(np.float64)
-    ref = og.logits.f32().astype(np.float64)
-    assert np.isfinite(got).all() and np.abs(got - ref).max() / np.abs(ref).max() < 3e-2
+    assert np.isfinite(got).all() and L.rel_err(got, og.logits.f32().astype(np.float64)) < 3e-2

@@ -105,7 +105,7 @@ def _repeat_kv_reference(kc, vc, q, k, v, pos):
 
 @pytest.mark.parametrize("G", [2, 4, 7, 32, 48])
 def test_oracle_head_mapping(G):
-    from tests.gqa_oracle import attention_kvcache_gqa
+    from tests.llama_oracle import attention_kvcache_gqa
     rng = np.random.default_rng(G)
     Bn, Hkv, S, pos = 2, 2, 40, 33
     kc = (rng.standard_normal((Bn, Hkv, S, 128)) * 0.5).astype(np.float32)
@@ -168,7 +168,7 @@ def _gqa_onnx_cfg(kv, dtype=F32):
 def test_gqa_onnx_roundtrip_schedule_and_oracle():
     """OnnxExporter -> OnnxStub of a GQA graph: same schedule on the C++ host, identical oracle bits"""
     from infinitensor_b200 import backend as B, graphs as G, onnx_lite as X
-    from tests.gqa_oracle import GqaOracleHandler
+    from tests.llama_oracle import LlamaOracleHandler
     rt = B.HostPlanRuntime()
     cfg = _gqa_onnx_cfg(2)
     h = B.GraphHandler(rt)
@@ -181,13 +181,13 @@ def test_gqa_onnx_roundtrip_schedule_and_oracle():
 
     small = G.LlamaConfig(layers=2, d_model=512, heads=4, kv_heads=1, head_dim=128, ffn=384, vocab=96, s_max=16, batch=3,
                           dtype=F32)
-    exp = X.OnnxExporter(GqaOracleHandler())
+    exp = X.OnnxExporter(LlamaOracleHandler())
     ge = G.build_llama_decode(exp, small)
     exp.data_malloc()
     G.fill_llama_weights_host(ge)
     blob = exp.save()
-    stub = X.OnnxStub(blob, handler=GqaOracleHandler())
-    oh = GqaOracleHandler()
+    stub = X.OnnxStub(blob, handler=LlamaOracleHandler())
+    oh = LlamaOracleHandler()
     gd = G.build_llama_decode(oh, small)
     oh.data_malloc()
     G.fill_llama_weights_host(gd)

@@ -152,19 +152,19 @@ def test_gpt2_decode_on_oracle_matches_forward(dtype):
     """token by token from an empty cache, the decode step reproduces the rows of build_gpt2's forward over the same
     tokens (the oracle executing both graphs)"""
     from infinitensor_b200 import graphs as G
-    from tests.head64_oracle import HeadWidthOracleHandler
+    from tests.llama_oracle import LlamaOracleHandler
     T = 20
     cfg = _gpt2_small_cfg(dtype, T)
     rng = np.random.default_rng(3)
     ids = rng.integers(0, cfg.vocab, size=(cfg.batch, T)).astype(np.int64)
-    fh = HeadWidthOracleHandler()
+    fh = LlamaOracleHandler()
     fg = G.build_gpt2(fh, cfg)
     G.fill_gpt2_weights_host(fg)
     fg.input_ids.copyin_numpy(ids)
     fg.position_ids.copyin_numpy(np.broadcast_to(np.arange(T, dtype=np.int64), (cfg.batch, T)).copy())
     fh.run()
     ref = fg.out.f32().astype(np.float64)  # [B, T, vocab]
-    dh = HeadWidthOracleHandler()
+    dh = LlamaOracleHandler()
     dg = G.build_gpt2_decode(dh, cfg, 32)
     G.fill_gpt2_weights_host(dg)
     for c in dg.k_caches + dg.v_caches:

@@ -65,7 +65,7 @@ def test_launcher_refuses_before_any_launch():
 @pytest.mark.parametrize("D,G,p,S,per_row", [(64, 4, [0, 5], 9, True), (128, 1, [3], 7, False), (128, 2, [0, 60], 4, True),
                                              (64, 1, [30], 34, False)])
 def test_oracle_loop_matches_float64_causal_attention(D, G, p, S, per_row):
-    from tests.prompt_oracle import attention_kvcache_prompt
+    from tests.llama_oracle import attention_kvcache_prompt
     Bn = len(p)
     # (scores up to 20: the oracle's 128-wide step exponentiates scores without subtracting their maximum, as the reference)
     c = prompt64.Case(Bn, 2 * G, 2, S, 64, p if per_row else p[0], D, seed=5, regimes=["flat", "late", "sink", "diag"])
@@ -89,7 +89,7 @@ def oracle_ulp(x):
 
 
 def test_prompt_starts_rules():
-    from tests.prompt_oracle import prompt_starts
+    from tests.llama_oracle import prompt_starts
     pos = np.array([[5, 6, 7], [40, 41, 42]])
     assert list(prompt_starts(pos, 2, 3, 64, True)) == [5, 40]
     assert list(prompt_starts(pos, 2, 3, 64, False)) == [5, 5]
@@ -98,23 +98,25 @@ def test_prompt_starts_rules():
 
 
 def test_single_token_oracle_unchanged():
-    """at S = 1 the prompt oracle handler is the grouped-query / head-width oracle, bit for bit"""
-    from infinitensor_b200 import graphs as G
-    from tests.head64_oracle import HeadWidthOracleHandler
-    from tests.prompt_oracle import PromptOracleHandler
-    cfg = G.LlamaConfig(layers=1, d_model=256, heads=4, kv_heads=2, head_dim=64, ffn=256, vocab=64, s_max=16, batch=2)
-    outs = []
-    for H in (HeadWidthOracleHandler, PromptOracleHandler):
-        h = H()
-        g = G.build_llama_decode(h, cfg)
-        _fill(g, cfg)
-        for i, t in enumerate(g.k_caches + g.v_caches):
-            t.copyin_numpy(G.to_storage(np.random.default_rng(i).standard_normal(t.dims).astype(np.float32), cfg.dtype))
-        g.input_ids.copyin_numpy(np.array([[3], [9]], np.int64))
-        g.position_ids.copyin_numpy(np.array([[4], [4]], np.int64))
-        h.run()
-        outs.append(g.logits.f32().copy())
-    assert np.array_equal(outs[0], outs[1])
+    """at S = 1 the oracle handler's AttentionKVCache is the single-token rule (64-wide grouped-query heads here): output and
+    cache writes bit for bit attention_kvcache_d's on the same arrays"""
+    import oracle
+    from tests.llama_oracle import LlamaOracleHandler, attention_kvcache_d
+    Bn, Hq, Hkv, Smax, D = 2, 8, 2, 16, 64
+    rng = np.random.default_rng(4)
+    vals = [oracle.round_to(rng.standard_normal(shape).astype(np.float32), BF16)
+            for shape in ((Bn, Hkv, Smax, D), (Bn, Hkv, Smax, D), (Bn, Hq, 1, D), (Bn, Hkv, 1, D), (Bn, Hkv, 1, D))]
+    h = LlamaOracleHandler()
+    ts = [h.tensor(list(a.shape), BF16) for a in vals]
+    for t, a in zip(ts, vals):
+        t.set_f32(a)
+    pos = h.tensor([Bn, 1], I64)
+    pos.copyin_numpy(np.array([[4], [4]], np.int64))
+    out = h.attentionKVCache(*ts, pos, None)
+    kc, vc = vals[0].copy(), vals[1].copy()
+    ref = attention_kvcache_d(kc, vc, *vals[2:], 4, BF16)
+    h.run()
+    assert np.array_equal(out.f32(), ref) and np.array_equal(ts[0].f32(), kc) and np.array_equal(ts[1].f32(), vc)
 
 
 # ---------------------------------------------------------------- the Llama prompt-step graph
@@ -198,7 +200,7 @@ def test_prompt_then_decode_equals_single_token_steps(head_dim, kv):
     single-token steps: the oracle's GEMMs, norms and RoPE compute every row on its own, and its AttentionKVCache over S
     tokens is S single-token steps by definition, so nothing depends on how the tokens are batched."""
     from infinitensor_b200 import graphs as G
-    from tests.prompt_oracle import PromptOracleHandler
+    from tests.llama_oracle import LlamaOracleHandler
     cfg = _cfg(head_dim=head_dim, kv_heads=kv, heads=4 if head_dim == 128 else 8, batch=2, dtype=BF16)
     S, p0 = 5, 3
     rng = np.random.default_rng(7)
@@ -207,7 +209,7 @@ def test_prompt_then_decode_equals_single_token_steps(head_dim, kv):
               for _ in range(2 * cfg.layers)]
 
     def graph(seq):
-        h = PromptOracleHandler()
+        h = LlamaOracleHandler()
         g = G.build_llama_decode(h, cfg, seq=seq)
         _fill(g, cfg)
         return h, g

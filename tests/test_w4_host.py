@@ -9,6 +9,7 @@ import pytest
 
 from tests import ref64
 from tests import w4_oracle as W
+from tests.llama_oracle import LlamaOracleHandler
 
 F32, U8, F16, BF16, I64 = 1, 2, 10, 16, 7
 
@@ -252,12 +253,12 @@ def test_onnx_round_trip_oracle_bit_identical():
     from infinitensor_b200 import graphs as G
     from infinitensor_b200 import onnx_lite as X
     cfg = _cfg(int4_block=32, batch=2)
-    exp, ge = _export(None, cfg, W.W4OracleHandler())
+    exp, ge = _export(None, cfg, LlamaOracleHandler())
     blob = exp.save()
-    oh = W.W4OracleHandler()
+    oh = LlamaOracleHandler()
     og = G.build_llama_decode(oh, cfg)
     G.fill_llama_weights_host(og)
-    ih = W.W4OracleHandler()
+    ih = LlamaOracleHandler()
     stub = X.OnnxStub(blob, handler=ih)
     rng = np.random.default_rng(3)
     feeds = {ge.input_ids.name: rng.integers(0, cfg.vocab, size=(cfg.batch, 1)).astype(np.int64),

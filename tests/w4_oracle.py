@@ -9,14 +9,12 @@ W[k, n] = (q[n, k] - z[n, k / bs]) * s[n, k / bs].
 * `reference` is the float64 product over the dequantised weights with the decode GEMMs' bound of tests/ref64.py,
   ulp_T(|ref|) + 2^-16 |A| . |W|;
 * `emulate32` follows the decode kernel's arithmetic in float32: per block a float32 partial sum of x . (q - z), folded into the
-  float32 accumulator as fma(partial, s, acc), one rounding to T.  `bugs` injects slips the bound must catch;
-* `W4OracleHandler` adds `matMulNBits` to the graph oracle: the decode rule for at most 64 rows, and for more rows the rule of
-  the dequantise-then-GEMM path (weights rounded to T once, then the 16-bit MatMul)."""
+  float32 accumulator as fma(partial, s, acc), one rounding to T.  `bugs` injects slips the bound must catch.
+The graph oracle's MatMulNBits (tests/llama_oracle.py) runs on `dequantize`."""
 import numpy as np
 
 import oracle as O
 from tests import ref64
-from tests.prompt_oracle import PromptOracleHandler
 
 F32, F16, BF16 = 1, 10, 16
 
@@ -108,20 +106,3 @@ def emulate32(x, b, scales, zp, K, N, bs, dt, bugs=()):
         acc = (part.astype(np.float64) * sc[None, :] + acc.astype(np.float64)).astype(f)  # one fma: exact in float64, one rounding
     return O.round_to(acc, dt)
 
-
-class W4OracleHandler(PromptOracleHandler):
-    """The graph oracle (grouped-query, head-width and prompt-chunk attention) with MatMulNBits."""
-
-    def matMulNBits(self, a, b, scales, zero_points, y, K, N, block_size, bits=4, g_idx=None, bias=None):
-        assert bits == 4 and g_idx is None and bias is None
-        out = self._out(y, list(a.dims[:-1]) + [N], a.dt)
-
-        def run():
-            x = np.asarray(a.value, np.float32).reshape(-1, K)
-            zp = None if zero_points is None else zero_points.value
-            w = dequantize(b.value, scales.value, zp, K, N, block_size)
-            if x.shape[0] > 64:  # dequantise to T, then the 16-bit MatMul
-                return O.matmul(x, O.round_to(w.astype(np.float32), a.dt), None, False, False, a.dt).reshape(out.dims)
-            return O.round_to((x.astype(np.float64) @ w).astype(np.float32), a.dt).reshape(out.dims)
-        ins = [a, b, scales] + ([] if zero_points is None else [zero_points])
-        return self._rec(run, ins, [out])
