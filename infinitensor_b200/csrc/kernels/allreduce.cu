@@ -180,11 +180,9 @@ extern "C" int it_b200_allreduce_fused(int dtype, const void *in, const void *re
     }
     ITB_DISPATCH_FLOAT(dtype, "allreduce_fused", {
         int threads = std::min(512, std::max(32, ((hidden / Vec16<T>::N + 31) / 32) * 32));
-        cudaError_t e = launch_k(allreduce_ll_kernel<T>, dim3(tokens), dim3(threads), 0, (cudaStream_t)stream, peers, world,
-                                 rank, (const T *)in, (const T *)residual, (const T *)norm_w, (T *)out, (T *)out_norm,
-                                 hidden, timeout_flag);
-        ITB_CHECK(e == cudaSuccess, "allreduce_fused: launch failed: %s", cudaGetErrorString(e));
+        return launch("allreduce_fused", allreduce_ll_kernel<T>, {dim3(tokens), dim3(threads), 0, (cudaStream_t)stream}, peers,
+                      world, rank, (const T *)in, (const T *)residual, (const T *)norm_w, (T *)out, (T *)out_norm, hidden,
+                      timeout_flag);
     });
-    ITB_LAUNCH_CHECK("allreduce_fused");
     return 0;
 }

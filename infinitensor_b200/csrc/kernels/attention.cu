@@ -1131,18 +1131,15 @@ static int launch_attn_stream(KT *kc, KT *vc, const T *q, const T *k, const T *v
                               float *workspace, const float *k_scale, const float *v_scale, cudaStream_t st) {
     constexpr int WARPS = 8, U = 4;  // consumer warps x rows per lane and chunk
     constexpr int CH = WARPS * RowCfg<KT, D>::RPW * U;
-    const size_t smem = (size_t)AS_STAGES * 2 * CH * D * sizeof(KT);
+    constexpr int smem = AS_STAGES * 2 * CH * D * (int)sizeof(KT);
+    constexpr const char *what = KV8<KT> ? "AttentionKVCache(FP8 cache): streaming kernel" : "AttentionKVCache: streaming kernel";
     int *tickets = stream_tickets(st, BH);
-    if (!tickets) return 1;
+    if (!tickets) ITB_FAIL("%s: no ticket pool", what);
     const int64_t max_units = (int64_t)BH * (S_max / CH + 1);
     const int grid = (int)std::min<int64_t>(max_units, (int64_t)AS_CTAS_PER_SM * kNumSMs);
     auto go = [&](auto kern, auto... scales) {  // scales: FP8 only
-        // the attribute is per DEVICE: a process may own runtimes on several GPUs
-        if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) return 1;
-        const cudaError_t e = launch_k(kern, dim3(grid), dim3((WARPS + 1) * 32), smem, st, kc, vc, q, k, v, position_id,
-                                       pos_flags, out, S_max, BH, workspace, stream_slots_per_head(S_max), tickets, rope_pos,
-                                       rope_pos_dtype, H, scales...);
-        return e == cudaSuccess ? 0 : 1;
+        return launch(what, kern, {dim3(grid), dim3((WARPS + 1) * 32), smem, st}, kc, vc, q, k, v, position_id, pos_flags, out,
+                      S_max, BH, workspace, stream_slots_per_head(S_max), tickets, rope_pos, rope_pos_dtype, H, scales...);
     };
     if constexpr (std::is_same_v<KT, uint8_t>) return go(attn_stream_kv8_kernel<T, D, WARPS, U, ROPE>, k_scale, v_scale);
     else return go(D == 128 ? attn_stream_kernel<T, WARPS, U, ROPE> : attn_stream64_kernel<T, WARPS, U, ROPE>);
@@ -1153,18 +1150,17 @@ static int launch_attn_gqa(KT *kc, KT *vc, const T *q, const T *k, const T *v, c
                            const void *rope_pos, int rope_pos_dtype, T *out, int B, int Hkv, int G, int S_max,
                            float *workspace, const float *k_scale, const float *v_scale, cudaStream_t st) {
     constexpr int CH = GqaCfg<T, D, KT>::CH;
-    const size_t smem = (size_t)AS_STAGES * 2 * CH * D * sizeof(KT);
+    constexpr int smem = AS_STAGES * 2 * CH * D * (int)sizeof(KT);
+    constexpr const char *what = KV8<KT> ? "AttentionKVCache(FP8 cache): grouped-query kernel" : "AttentionKVCache: grouped-query kernel";
     const int nqg = (G + 16 * QT - 1) / (16 * QT);  // query groups per KV head
     int *tickets = stream_tickets(st, B * Hkv * nqg);
-    if (!tickets) return 1;
+    if (!tickets) ITB_FAIL("%s: no ticket pool", what);
     const int64_t max_units = (int64_t)B * Hkv * nqg * (S_max / CH + 1);
     const int grid = (int)std::min<int64_t>(max_units, (int64_t)AS_CTAS_PER_SM * kNumSMs);
     auto go = [&](auto kern, auto... scales) {  // scales: FP8 only
-        if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) return 1;
-        const cudaError_t e = launch_k(kern, dim3(grid), dim3((GQ_WARPS + 1) * 32), smem, st, kc, vc, q, k, v, position_id,
-                                       pos_flags, out, S_max, B, Hkv, G, nqg, workspace, stream_slots_per_head(S_max), tickets,
-                                       rope_pos, rope_pos_dtype, scales...);
-        return e == cudaSuccess ? 0 : 1;
+        return launch(what, kern, {dim3(grid), dim3((GQ_WARPS + 1) * 32), smem, st}, kc, vc, q, k, v, position_id, pos_flags,
+                      out, S_max, B, Hkv, G, nqg, workspace, stream_slots_per_head(S_max), tickets, rope_pos, rope_pos_dtype,
+                      scales...);
     };
     if constexpr (std::is_same_v<KT, uint8_t>) return go(attn_gqa_kv8_kernel<T, D, QT, ROPE>, k_scale, v_scale);
     else return go(D == 128 ? attn_gqa_kernel<T, QT, ROPE> : attn_gqa64_kernel<T, QT, ROPE>);
@@ -1223,25 +1219,18 @@ static int attention_impl(int dtype, void *k_cache, void *v_cache, const void *q
         ITB_CHECK(v_scale, "AttentionKVCache(FP8 cache): the V scale is missing");
         ITB_CHECK(((reinterpret_cast<uintptr_t>(k_scale) | reinterpret_cast<uintptr_t>(v_scale)) & 3) == 0,
                   "AttentionKVCache(FP8 cache): scales must be 4-byte aligned");
-        auto launch = [&](auto tag) {
+        auto fp8 = [&](auto tag) {
             using T = decltype(tag);
             auto go = D == 64 ? launch_attn_width<T, uint8_t, 64> : launch_attn_width<T, uint8_t, 128>;
             return go((uint8_t *)k_cache, (uint8_t *)v_cache, (const T *)q, (const T *)k, (const T *)v, position_id, pos_flags,
                       rope_pos, rope_pos_dtype, (T *)out, B, Hq, Hkv, S_max, (float *)workspace, k_scale, v_scale, st);
         };
-        const int rc = dtype == ITB_F16 ? launch(__half{}) : launch(__nv_bfloat16{});
-        ITB_CHECK(rc == 0, "AttentionKVCache(FP8 cache): %s kernel launch failed: %s", Hq > Hkv ? "grouped-query" : "streaming",
-                  cudaGetErrorString(cudaGetLastError()));
-        ITB_LAUNCH_CHECK("AttentionKVCache");
-        return 0;
+        return dtype == ITB_F16 ? fp8(__half{}) : fp8(__nv_bfloat16{});
     }
     ITB_DISPATCH_FLOAT(dtype, "AttentionKVCache", {
         auto go = D == 64 ? launch_attn_width<T, T, 64> : launch_attn_width<T, T, 128>;
-        int rc = go((T *)k_cache, (T *)v_cache, (const T *)q, (const T *)k, (const T *)v, position_id, pos_flags, rope_pos,
-                    rope_pos_dtype, (T *)out, B, Hq, Hkv, S_max, (float *)workspace, nullptr, nullptr, st);
-        ITB_CHECK(rc == 0, "AttentionKVCache: %s kernel launch failed: %s", Hq > Hkv ? "grouped-query" : "streaming",
-                  cudaGetErrorString(cudaGetLastError()));
-        ITB_LAUNCH_CHECK("AttentionKVCache");
+        return go((T *)k_cache, (T *)v_cache, (const T *)q, (const T *)k, (const T *)v, position_id, pos_flags, rope_pos,
+                  rope_pos_dtype, (T *)out, B, Hq, Hkv, S_max, (float *)workspace, nullptr, nullptr, st);
     });
     return 0;
 }

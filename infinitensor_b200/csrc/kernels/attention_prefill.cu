@@ -378,21 +378,8 @@ static int launch_ap(const void *q, const void *k, const void *v, ApArgs a, cuda
             ITB_FAIL("attention_prefill: cuTensorMapEncodeTiled (strided views) failed");
     }
     const int smem = 2 * AP_BQ * D * 2 + AP_BK * D * 2 + AP_BQ * AP_BK * 2 + AP_BK * AP_MPAD * 2 + AP_BK * AP_SLD * 2 + 1024;
-    auto kern = attention_prefill_kernel<T, D>;
-    static int attr_smem[64] = {0};  // per device
-    int dev = 0;
-    cudaGetDevice(&dev);
-    dev &= 63;
-    cudaError_t e = cudaSuccess;
-    if (smem > attr_smem[dev]) {
-        e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-        ITB_CHECK(e == cudaSuccess, "attention_prefill: smem attribute: %s", cudaGetErrorString(e));
-        attr_smem[dev] = smem;
-    }
-    e = launch_k(kern, dim3((a.Sq + AP_BQ - 1) / AP_BQ, a.BH), dim3(AP_THREADS), (size_t)smem, st, mq, mk, mv, a);
-    ITB_CHECK(e == cudaSuccess, "attention_prefill: launch failed: %s", cudaGetErrorString(e));
-    ITB_LAUNCH_CHECK("attention_prefill");
-    return 0;
+    return launch("attention_prefill", attention_prefill_kernel<T, D>,
+                  {dim3((a.Sq + AP_BQ - 1) / AP_BQ, a.BH), dim3(AP_THREADS), smem, st}, mq, mk, mv, a);
 }
 
 // ------------------------------------------------------------------------------------------------------------------
@@ -629,22 +616,18 @@ template <typename T, int D>
 static int launch_prompt(void *kc, void *vc, const void *q, const void *k, const void *v, const PkArgs &a, int B,
                          cudaStream_t st) {
     const int64_t chunks = (int64_t)a.S * D / 8;
-    cudaError_t e = launch_k(kvcache_append_kernel<T>, dim3((unsigned)((chunks + 255) / 256), B * a.Hkv), dim3(256), (size_t)0, st,
-                             (T *)kc, (T *)vc, (const T *)k, (const T *)v, a.pos, a.pos_flags, a.Hkv, a.S, a.Smax, D);
-    ITB_CHECK(e == cudaSuccess, "AttentionKVCache prompt: append launch failed: %s", cudaGetErrorString(e));
+    if (launch("AttentionKVCache prompt: append", kvcache_append_kernel<T>,
+               {dim3((unsigned)((chunks + 255) / 256), B * a.Hkv), dim3(256), 0, st}, (T *)kc, (T *)vc, (const T *)k, (const T *)v,
+               a.pos, a.pos_flags, a.Hkv, a.S, a.Smax, D))
+        return 1;
     CUtensorMap mq, mk, mv;
     if (!make_tma_3d_b16(&mq, q, (uint64_t)B * a.Hq, (uint64_t)a.S, D, D, (uint64_t)a.S * D, PK_BQ, 64) ||
         !make_tma_3d_b16(&mk, kc, (uint64_t)B * a.Hkv, (uint64_t)a.Smax, D, D, (uint64_t)a.Smax * D, PK_BK, 64) ||
         !make_tma_3d_b16(&mv, vc, (uint64_t)B * a.Hkv, (uint64_t)a.Smax, D, D, (uint64_t)a.Smax * D, PK_BK, 64))
         ITB_FAIL("AttentionKVCache prompt: cuTensorMapEncodeTiled failed");
     const int smem = 5 * PK_BQ * D * 2 + 2 * PK_BQ * PK_BK * 2 + 1024;
-    auto kern = attention_kvcache_prompt_kernel<T, D>;
-    e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-    ITB_CHECK(e == cudaSuccess, "AttentionKVCache prompt: smem attribute: %s", cudaGetErrorString(e));
-    e = launch_k(kern, dim3((a.S + PK_BQ - 1) / PK_BQ, B * a.Hq), dim3(PK_THREADS), (size_t)smem, st, mq, mk, mv, a);
-    ITB_CHECK(e == cudaSuccess, "AttentionKVCache prompt: launch failed: %s", cudaGetErrorString(e));
-    ITB_LAUNCH_CHECK("AttentionKVCache prompt");
-    return 0;
+    return launch("AttentionKVCache prompt", attention_kvcache_prompt_kernel<T, D>,
+                  {dim3((a.S + PK_BQ - 1) / PK_BQ, B * a.Hq), dim3(PK_THREADS), smem, st}, mq, mk, mv, a);
 }
 
 }  // namespace itb

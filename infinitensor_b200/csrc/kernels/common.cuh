@@ -14,7 +14,6 @@ namespace itb {
 
 // ---- error reporting (the C spelling of infini::Exception) -------------------------------
 void set_error(const char *fmt, ...);
-void count_launch(int n = 1);
 
 #define ITB_FAIL(...)                                                                          \
     do {                                                                                       \
@@ -25,13 +24,6 @@ void count_launch(int n = 1);
 #define ITB_CHECK(cond, ...)                                                                   \
     do {                                                                                       \
         if (!(cond)) ITB_FAIL(__VA_ARGS__);                                                    \
-    } while (0)
-
-#define ITB_LAUNCH_CHECK(name)                                                                 \
-    do {                                                                                       \
-        cudaError_t e__ = cudaPeekAtLastError();                                               \
-        if (e__ != cudaSuccess) ITB_FAIL("%s: launch failed: %s", name, cudaGetErrorString(e__)); \
-        itb::count_launch();                                                                   \
     } while (0)
 
 constexpr int kNumSMs = 132;  // H100 SXM
@@ -48,20 +40,46 @@ bool pdl_enabled();  // false when ITB_NO_PDL=1
 // zero-initialised, self-cleaning int tickets private to (device, stream); nullptr if n exceeds the pool (65536)
 int *stream_tickets(cudaStream_t st, int n);
 
+// ---- the one kernel launch path ------------------------------------------------------------
+struct LaunchCfg {
+    dim3 grid, block;
+    int smem;  // dynamic shared memory, bytes
+    cudaStream_t stream;
+    dim3 cluster = dim3(0, 0, 0);  // x == 0: no cluster attribute
+};
+// raises `kernel`'s dynamic shared-memory limit on the current device to `smem` unless it already allows that much;
+// 0, or 1 with the error set
+int opt_in_smem(const char *what, const void *kernel, int smem);
+// the result of one cudaLaunchKernelEx: counts the launch (0), or sets "<what>: <CUDA error>" (1)
+int launched(const char *what, cudaError_t e);
+
+// Every kernel goes through here: its shared memory opted in, the cluster attribute when given, PDL unless ITB_NO_PDL=1,
+// and one count in it_b200_launch_count() per kernel launched.  0, or 1 with the error set.
 template <typename... KArgs, typename... Args>
-inline cudaError_t launch_k(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st,
-                            Args &&...args) {
+inline int launch(const char *what, void (*kernel)(KArgs...), const LaunchCfg &c, Args &&...args) {
+    if (c.smem > 0 && opt_in_smem(what, reinterpret_cast<const void *>(kernel), c.smem)) return 1;
     cudaLaunchConfig_t cfg{};
-    cfg.gridDim = grid;
-    cfg.blockDim = block;
-    cfg.dynamicSmemBytes = smem;
-    cfg.stream = st;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[0].val.programmaticStreamSerializationAllowed = 1;
+    cfg.gridDim = c.grid;
+    cfg.blockDim = c.block;
+    cfg.dynamicSmemBytes = (size_t)c.smem;
+    cfg.stream = c.stream;
+    cudaLaunchAttribute attr[2];
+    unsigned n = 0;
+    if (c.cluster.x) {
+        attr[n].id = cudaLaunchAttributeClusterDimension;
+        attr[n].val.clusterDim.x = c.cluster.x;
+        attr[n].val.clusterDim.y = c.cluster.y;
+        attr[n].val.clusterDim.z = c.cluster.z;
+        ++n;
+    }
+    if (pdl_enabled()) {
+        attr[n].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+        attr[n].val.programmaticStreamSerializationAllowed = 1;
+        ++n;
+    }
     cfg.attrs = attr;
-    cfg.numAttrs = pdl_enabled() ? 1 : 0;
-    return cudaLaunchKernelEx(&cfg, kernel, std::forward<Args>(args)...);
+    cfg.numAttrs = n;
+    return launched(what, cudaLaunchKernelEx(&cfg, kernel, std::forward<Args>(args)...));
 }
 
 inline int dtype_size(int dt) {

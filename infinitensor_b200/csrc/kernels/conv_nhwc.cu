@@ -547,22 +547,8 @@ static int launch_conv_nhwc_t(bool is_bf16, const void *x, const void *wk, int C
     if (!make_tma_2d_b16(&mapY, ymat, yrows, ycols, ycols, 32, 32, 64) || !make_tma_2d_b16(&mapR, rmat, yrows, ycols, ycols, 32, 32, 64))
         ITB_FAIL("conv(nhwc): cuTensorMapEncodeTiled(output) failed");
 
-    auto kern = conv_nhwc_kernel<T, CV_FT>;
-    {
-        static int attr_smem[64] = {0};
-        int dev = 0;
-        cudaGetDevice(&dev);
-        dev &= 63;
-        if (smem > attr_smem[dev]) {
-            cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-            ITB_CHECK(e == cudaSuccess, "conv(nhwc): smem attribute: %s", cudaGetErrorString(e));
-            attr_smem[dev] = smem;
-        }
-    }
-    cudaError_t e = launch_k(kern, dim3(std::min(p.tiles, kNumSMs)), dim3(CV_THREADS), (size_t)smem, st, mapA, mapB, mapY, mapR, p);
-    ITB_CHECK(e == cudaSuccess, "conv(nhwc): launch failed: %s", cudaGetErrorString(e));
-    count_launch();
-    return 0;
+    return launch("conv(nhwc)", conv_nhwc_kernel<T, CV_FT>, {dim3(std::min(p.tiles, kNumSMs)), dim3(CV_THREADS), smem, st}, mapA,
+                  mapB, mapY, mapR, p);
 }
 
 }  // namespace itb
@@ -609,21 +595,20 @@ extern "C" int it_b200_conv2d_nhwc(int dtype, const void *x, const void *w, void
         ITB_CHECK(workspace && workspace_bytes >= need && aligned16(workspace), "conv(nhwc): workspace %lld < %lld bytes",
                   (long long)workspace_bytes, (long long)need);
         const int64_t total = (int64_t)F * R * S * Cp;
-        if (R * S == 9) {
-            const int64_t items = (int64_t)F * (Cp / 8);
-            if (dtype == ITB_F16)
-                launch_k(repack_filters9_kernel<__half>, dim3(grid_for(items, 256)), dim3(256), 0, st, (const __half *)w,
-                         (__half *)workspace, items, C, Cp);
-            else
-                launch_k(repack_filters9_kernel<__nv_bfloat16>, dim3(grid_for(items, 256)), dim3(256), 0, st, (const __nv_bfloat16 *)w,
-                         (__nv_bfloat16 *)workspace, items, C, Cp);
-        } else if (dtype == ITB_F16)
-            launch_k(repack_filters_kernel<__half>, dim3(grid_for(total, 256)), dim3(256), 0, st, (const __half *)w,
-                     (__half *)workspace, total, C, R * S, Cp);
+        const char *what = "conv(nhwc): filter repack";
+        const int64_t items = R * S == 9 ? (int64_t)F * (Cp / 8) : total;
+        const LaunchCfg c{dim3(grid_for(items, 256)), dim3(256), 0, st};
+        int rc;
+        if (R * S == 9)
+            rc = dtype == ITB_F16 ? launch(what, repack_filters9_kernel<__half>, c, (const __half *)w, (__half *)workspace, items, C, Cp)
+                                  : launch(what, repack_filters9_kernel<__nv_bfloat16>, c, (const __nv_bfloat16 *)w,
+                                           (__nv_bfloat16 *)workspace, items, C, Cp);
         else
-            launch_k(repack_filters_kernel<__nv_bfloat16>, dim3(grid_for(total, 256)), dim3(256), 0, st, (const __nv_bfloat16 *)w,
-                     (__nv_bfloat16 *)workspace, total, C, R * S, Cp);
-        ITB_LAUNCH_CHECK("conv(nhwc): filter repack");
+            rc = dtype == ITB_F16 ? launch(what, repack_filters_kernel<__half>, c, (const __half *)w, (__half *)workspace, total, C,
+                                           R * S, Cp)
+                                  : launch(what, repack_filters_kernel<__nv_bfloat16>, c, (const __nv_bfloat16 *)w,
+                                           (__nv_bfloat16 *)workspace, total, C, R * S, Cp);
+        if (rc) return 1;
         wk = workspace;
     }
     if (dtype == ITB_F16)
@@ -652,11 +637,10 @@ extern "C" int it_b200_conv_repack_filters(int dtype, int n, const void *const *
             b.Cp[i] = nhwc_cp(C[j], R[j], S[j]);
             most = std::max<int64_t>(most, (int64_t)F[j] * b.RS[i] * b.Cp[i] / (b.RS[i] == 9 ? 72 : 1));
         }
-        const dim3 grid((unsigned)std::min<int64_t>((most + 255) / 256, 2 * kNumSMs), (unsigned)cnt);
-        cudaError_t e = dtype == ITB_F16 ? launch_k(repack_filters_batch_kernel<__half>, grid, dim3(256), 0, st, b)
-                                         : launch_k(repack_filters_batch_kernel<__nv_bfloat16>, grid, dim3(256), 0, st, b);
-        ITB_CHECK(e == cudaSuccess, "conv_repack_filters: launch failed: %s", cudaGetErrorString(e));
-        count_launch();
+        const LaunchCfg c{dim3((unsigned)std::min<int64_t>((most + 255) / 256, 2 * kNumSMs), (unsigned)cnt), dim3(256), 0, st};
+        const int rc = dtype == ITB_F16 ? launch("conv_repack_filters", repack_filters_batch_kernel<__half>, c, b)
+                                        : launch("conv_repack_filters", repack_filters_batch_kernel<__nv_bfloat16>, c, b);
+        if (rc) return 1;
     }
     return 0;
 }

@@ -170,22 +170,9 @@ static int stem_smem(const StemParams &p) {
 
 template <typename T>
 static int launch_stem_t(const StemParams &p, int smem, int64_t tiles, cudaStream_t st) {
-    auto kern = conv_stem_kernel<T>;
-    static int attr_smem[64] = {0};  // per device
-    int dev = 0;
-    cudaGetDevice(&dev);
-    dev &= 63;
-    if (smem > attr_smem[dev]) {
-        cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-        ITB_CHECK(e == cudaSuccess, "conv(stem): smem attribute: %s", cudaGetErrorString(e));
-        attr_smem[dev] = smem;
-    }
     const int ctas_per_sm = std::max(1, std::min(2, (220 * 1024) / (smem + 1024)));
-    cudaError_t e = launch_k(kern, dim3((unsigned)std::min<int64_t>(tiles, (int64_t)kNumSMs * ctas_per_sm)), dim3(ST_THREADS),
-                             (size_t)smem, st, p);
-    ITB_CHECK(e == cudaSuccess, "conv(stem): launch failed: %s", cudaGetErrorString(e));
-    count_launch();
-    return 0;
+    return launch("conv(stem)", conv_stem_kernel<T>,
+                  {dim3((unsigned)std::min<int64_t>(tiles, (int64_t)kNumSMs * ctas_per_sm)), dim3(ST_THREADS), smem, st}, p);
 }
 
 }  // namespace itb

@@ -261,10 +261,9 @@ extern "C" int it_b200_dequantize_fp8(int dtype_out, const void *xq, const float
     const int64_t n = rows * cols;
     if (n == 0) return 0;
     ITB_DISPATCH_FLOAT(dtype_out, "dequantize_fp8", {
-        launch_k(dequant_fp8_kernel<T>, dim3(grid_for(n, 256)), dim3(256), 0, (cudaStream_t)stream, (const uint8_t *)xq, scale, (T *)y,
-                 n, cols);
+        return launch("dequantize_fp8", dequant_fp8_kernel<T>, {dim3(grid_for(n, 256)), dim3(256), 0, (cudaStream_t)stream},
+                      (const uint8_t *)xq, scale, (T *)y, n, cols);
     });
-    ITB_LAUNCH_CHECK("dequantize_fp8");
     return 0;
 }
 
@@ -275,9 +274,9 @@ extern "C" int it_b200_unary_alpha(int op, int dtype, const void *x, void *y, in
     ITB_DISPATCH_FLOAT(dtype, "unary", {
         bool vec = aligned16(x) && aligned16(y);
         int64_t items = vec ? (n + Vec16<T>::N - 1) / Vec16<T>::N : n;
-        launch_k(unary_kernel<T>, dim3(grid_for(items, 256)), dim3(256), 0, st, op, (const T *)x, (T *)y, n, vec, alpha);
+        return launch("unary", unary_kernel<T>, {dim3(grid_for(items, 256)), dim3(256), 0, st}, op, (const T *)x, (T *)y, n, vec,
+                      alpha);
     });
-    ITB_LAUNCH_CHECK("unary");
     return 0;
 }
 extern "C" int it_b200_unary(int op, int dtype, const void *x, void *y, int64_t n, void *stream) {
@@ -290,10 +289,9 @@ extern "C" int it_b200_silu_mul(int dtype, const void *gate, const void *up, voi
     ITB_DISPATCH_FLOAT(dtype, "silu_mul", {
         bool vec = aligned16(gate) && aligned16(up) && aligned16(out);
         int64_t items = vec ? (n + Vec16<T>::N - 1) / Vec16<T>::N : n;
-        launch_k(silu_mul_kernel<T>, dim3(grid_for(items, 256)), dim3(256), 0, (cudaStream_t)stream, (const T *)gate,
-                 (const T *)up, (T *)out, n, vec);
+        return launch("silu_mul", silu_mul_kernel<T>, {dim3(grid_for(items, 256)), dim3(256), 0, (cudaStream_t)stream},
+                      (const T *)gate, (const T *)up, (T *)out, n, vec);
     });
-    ITB_LAUNCH_CHECK("silu_mul");
     return 0;
 }
 
@@ -315,23 +313,18 @@ extern "C" int it_b200_binary(int op, int dtype, const void *a, const void *b, v
         if (flat) {
             bool vec = aligned16(a) && aligned16(b) && aligned16(c);
             int64_t items = vec ? (n + Vec16<T>::N - 1) / Vec16<T>::N : n;
-            launch_k(binary_flat_kernel<T>, dim3(grid_for(items, 256)), dim3(256), 0, st, op, (const T *)a, (const T *)b, (T *)c, n, (int)cs[0].v[0], (int)cs[1].v[0], vec);
-        } else if (cmp) {
-            launch_k(binary_general_kernel<T, uint8_t>, dim3(grid_for(n, 256)), dim3(256), 0, st, op, (const T *)a, (const T *)b, (uint8_t *)c, n, cr, cd, cs[0], cs[1]);
-        } else {
-            launch_k(binary_general_kernel<T, T>, dim3(grid_for(n, 256)), dim3(256), 0, st, op, (const T *)a, (const T *)b, (T *)c, n, cr, cd, cs[0], cs[1]);
+            return launch("binary", binary_flat_kernel<T>, {dim3(grid_for(items, 256)), dim3(256), 0, st}, op, (const T *)a, (const T *)b, (T *)c, n, (int)cs[0].v[0], (int)cs[1].v[0], vec);
         }
+        const LaunchCfg cfg{dim3(grid_for(n, 256)), dim3(256), 0, st};
+        if (cmp)
+            return launch("binary", binary_general_kernel<T, uint8_t>, cfg, op, (const T *)a, (const T *)b, (uint8_t *)c, n, cr, cd, cs[0], cs[1]);
+        return launch("binary", binary_general_kernel<T, T>, cfg, op, (const T *)a, (const T *)b, (T *)c, n, cr, cd, cs[0], cs[1]);
     });
-    ITB_LAUNCH_CHECK("binary");
     return 0;
 }
 
 #define CAST_CASE(FROM, TO, SRC, DST)                                                          \
-    if (from == FROM && to == TO) {                                                            \
-        launch_k(cast_kernel<SRC, DST>, dim3(g), dim3(256), 0, st, (const SRC *)x, (DST *)y, n);                 \
-        ITB_LAUNCH_CHECK("cast");                                                              \
-        return 0;                                                                              \
-    }
+    if (from == FROM && to == TO) return launch("cast", cast_kernel<SRC, DST>, {dim3(g), dim3(256), 0, st}, (const SRC *)x, (DST *)y, n);
 
 extern "C" int it_b200_cast(int from, int to, const void *x, void *y, int64_t n, void *stream) {
     if (n == 0) return 0;
@@ -378,10 +371,9 @@ extern "C" int it_b200_where(int elem_size, const void *cond, const void *x, con
     const int64_t *strides[3] = {stride_c, stride_x, stride_y};
     int cr = collapse(rank, dims, strides, 3, cd, cs);
     ELEM_DISPATCH(elem_size, "where", {
-        launch_k(where_kernel<E>, dim3(grid_for(n, 256)), dim3(256), 0, st, (const uint8_t *)cond, (const E *)x, (const E *)y,
-                                                          (E *)out, n, cr, cd, cs[0], cs[1], cs[2]);
+        return launch("where", where_kernel<E>, {dim3(grid_for(n, 256)), dim3(256), 0, st}, (const uint8_t *)cond, (const E *)x,
+                      (const E *)y, (E *)out, n, cr, cd, cs[0], cs[1], cs[2]);
     });
-    ITB_LAUNCH_CHECK("where");
     return 0;
 }
 
@@ -396,8 +388,7 @@ extern "C" int it_b200_expand(int elem_size, const void *x, void *y, int rank, c
     const int64_t *strides[1] = {stride_x};
     int cr = collapse(rank, dims, strides, 1, cd, cs);
     ELEM_DISPATCH(elem_size, "expand", {
-        launch_k(expand_kernel<E>, dim3(grid_for(n, 256)), dim3(256), 0, st, (const E *)x, (E *)y, n, cr, cd, cs[0]);
+        return launch("expand", expand_kernel<E>, {dim3(grid_for(n, 256)), dim3(256), 0, st}, (const E *)x, (E *)y, n, cr, cd, cs[0]);
     });
-    ITB_LAUNCH_CHECK("expand");
     return 0;
 }

@@ -358,20 +358,21 @@ static int conv_impl(int dtype, const void *x, const void *w, void *y, int N, in
         const int64_t rowlen = fold ? (int64_t)N * P : P;
         ITB_DISPATCH_FLOAT(dtype, "conv(im2col)", {
             auto go = [&](auto kern, int64_t items) {
-                return launch_k(kern, dim3(grid_for(items, 256)), dim3(256), 0, st, (const T *)x, (T *)workspace, total, N, C, H,
-                                W, R, S, OH, OW, ph, pw, sh, sw, dh, dw);
+                return launch("conv(im2col)", kern, {dim3(grid_for(items, 256)), dim3(256), 0, st}, (const T *)x, (T *)workspace,
+                              total, N, C, H, W, R, S, OH, OW, ph, pw, sh, sw, dh, dw);
             };
+            int rc;
             if constexpr (sizeof(T) == 2) {
                 if (rowlen % 8 == 0 && aligned16(workspace)) {
-                    if (fold) go(im2col_kernel<T, true, true>, total / 8); else go(im2col_kernel<T, false, true>, total / 8);
+                    rc = fold ? go(im2col_kernel<T, true, true>, total / 8) : go(im2col_kernel<T, false, true>, total / 8);
                 } else {
-                    if (fold) go(im2col_kernel<T, true, false>, total); else go(im2col_kernel<T, false, false>, total);
+                    rc = fold ? go(im2col_kernel<T, true, false>, total) : go(im2col_kernel<T, false, false>, total);
                 }
             } else {
-                if (fold) go(im2col_kernel<T, true, false>, total); else go(im2col_kernel<T, false, false>, total);
+                rc = fold ? go(im2col_kernel<T, true, false>, total) : go(im2col_kernel<T, false, false>, total);
             }
+            if (rc) return 1;
         });
-        ITB_LAUNCH_CHECK("conv(im2col)");
         col = workspace;
     }
     if (fold) {
@@ -381,10 +382,10 @@ static int conv_impl(int dtype, const void *x, const void *w, void *y, int N, in
             char *wpad = (char *)workspace + (((int64_t)N * Kp * P * es + 255) & ~255ll);
             const int64_t wt = (int64_t)F * Kp;
             ITB_DISPATCH_FLOAT(dtype, "conv(pad filters)", {
-                launch_k(pad_rows_kernel<T>, dim3(grid_for(wt, 256)), dim3(256), 0, st, (const T *)w, (T *)wpad, wt, (int)Kc,
-                         (int)Kp);
+                if (launch("conv(pad filters)", pad_rows_kernel<T>, {dim3(grid_for(wt, 256)), dim3(256), 0, st}, (const T *)w,
+                           (T *)wpad, wt, (int)Kc, (int)Kp))
+                    return 1;
             });
-            ITB_LAUNCH_CHECK("conv(pad filters)");
             wmat = wpad;
         }
         GemmArgs g{};

@@ -81,8 +81,7 @@ int launch_gemm_simt(int dtype, const GemmArgs &g, cudaStream_t st) {
     dim3 grid((g.n + 63) / 64, (g.m + 63) / 64, (unsigned)g.batch);
     ITB_CHECK(grid.y < 65536 && grid.z < 65536, "matmul(simt): grid too large (m=%d, batch=%lld)", g.m,
               (long long)g.batch);
-    ITB_DISPATCH_FLOAT(dtype, "matmul(simt)", { launch_k(gemm_simt_kernel<T>, dim3(grid), dim3(256), 0, st, g); });
-    ITB_LAUNCH_CHECK("matmul(simt)");
+    ITB_DISPATCH_FLOAT(dtype, "matmul(simt)", { return launch("matmul(simt)", gemm_simt_kernel<T>, {grid, dim3(256), 0, st}, g); });
     return 0;
 }
 

@@ -314,37 +314,9 @@ static int launch_skinny_nb(const GemmArgs &g, int ngroups, const void *const *W
     constexpr int stages_split = W8 ? stages_deep : Cfg::stages_for(kSkinnySplitBudgetKB);
     const int stages = splitk > 1 ? stages_split : stages_deep;
     const int smem_bytes = Cfg::smem_for(stages);
-    auto kern = gemm_skinny_kernel<T, MT, NB, W8>;
-    {
-        // the attribute is per DEVICE (a process may own runtimes on several GPUs): remember the largest request per device
-        static int attr_smem[64] = {0};  // (one table per template instantiation)
-        int dev = 0;
-        cudaGetDevice(&dev);
-        dev &= 63;
-        if (smem_bytes > attr_smem[dev]) {
-            cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes);
-            ITB_CHECK(e == cudaSuccess, "matmul(skinny): smem attribute: %s", cudaGetErrorString(e));
-            attr_smem[dev] = smem_bytes;
-        }
-    }
-    cudaLaunchConfig_t cfg{};
-    cfg.gridDim = dim3(tiles_n, splitk, 1);
-    cfg.blockDim = dim3(SK_THREADS, 1, 1);
-    cfg.dynamicSmemBytes = smem_bytes;
-    cfg.stream = st;
-    cudaLaunchAttribute attr[2];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = 1;
-    attr[0].val.clusterDim.y = splitk;
-    attr[0].val.clusterDim.z = 1;
-    attr[1].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[1].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = pdl_enabled() ? 2 : 1;
-    cudaError_t e = cudaLaunchKernelEx(&cfg, kern, grp, mapX, g, ktiles, per, stages);
-    ITB_CHECK(e == cudaSuccess, "matmul(skinny): launch failed: %s", cudaGetErrorString(e));
-    itb::count_launch();
-    return 0;
+    return launch("matmul(skinny)", gemm_skinny_kernel<T, MT, NB, W8>,
+                  {dim3(tiles_n, splitk, 1), dim3(SK_THREADS, 1, 1), smem_bytes, st, dim3(1, splitk, 1)}, grp, mapX, g, ktiles,
+                  per, stages);
 }
 
 // tile width: 128 columns once 64-wide tiles would already oversubscribe the 2 x 132 CTA slots

@@ -447,36 +447,9 @@ static int launch_tc_t(const GemmArgs &g, cudaStream_t st, bool is_bf16, int ngr
 
     auto kern = p.mpad == 16 ? gemm_tc_kernel<T, 16> : p.mpad == 32 ? gemm_tc_kernel<T, 32> : p.mpad == 64 ? gemm_tc_kernel<T, 64>
                                                                                                 : gemm_tc_kernel<T, 128>;
-    {
-        static int attr_smem[64][4] = {{0}};  // per device (see gemm_skinny.cu) and instance
-        int dev = 0;
-        cudaGetDevice(&dev);
-        dev &= 63;
-        const int ki = p.mpad == 16 ? 0 : p.mpad == 32 ? 1 : p.mpad == 64 ? 2 : 3;
-        if (smem > attr_smem[dev][ki]) {
-            cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-            ITB_CHECK(e == cudaSuccess, "matmul(wgmma): smem attribute: %s", cudaGetErrorString(e));
-            attr_smem[dev][ki] = smem;
-        }
-    }
-    cudaLaunchConfig_t cfg{};
-    cfg.gridDim = dim3(tiles_n, splitk, (unsigned)(g.batch * p.m_chunks));
-    cfg.blockDim = dim3(TC_THREADS, 1, 1);
-    cfg.dynamicSmemBytes = smem;
-    cfg.stream = st;
-    cudaLaunchAttribute attr[2];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = 1;
-    attr[0].val.clusterDim.y = splitk;
-    attr[0].val.clusterDim.z = 1;
-    attr[1].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[1].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = pdl_enabled() ? 2 : 1;
-    cudaError_t e = cudaLaunchKernelEx(&cfg, kern, grp, mapX, g, p);
-    ITB_CHECK(e == cudaSuccess, "matmul(wgmma): launch failed: %s", cudaGetErrorString(e));
-    itb::count_launch();
-    return 0;
+    return launch("matmul(wgmma)", kern,
+                  {dim3(tiles_n, splitk, (unsigned)(g.batch * p.m_chunks)), dim3(TC_THREADS, 1, 1), smem, st, dim3(1, splitk, 1)},
+                  grp, mapX, g, p);
 }
 
 int launch_gemm_tc(int dtype, const GemmArgs &g, cudaStream_t st) {

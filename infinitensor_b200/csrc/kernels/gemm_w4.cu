@@ -371,36 +371,9 @@ static int launch_w4(const void *X, int ngroups, const void *const *Wq, const vo
     constexpr int stages_deep = Cfg::stages_for(kW4DeepBudgetKB), stages_split = Cfg::stages_for(kW4SplitBudgetKB);
     const int stages = splitk > 1 ? stages_split : stages_deep;
     const int smem_bytes = Cfg::smem_for(stages);
-    auto kern = gemm_skinny_w4_kernel<T, MT, BS, ZP>;
-    {
-        static int attr_smem[64] = {0};  // per device, per instantiation
-        int dev = 0;
-        cudaGetDevice(&dev);
-        dev &= 63;
-        if (smem_bytes > attr_smem[dev]) {
-            cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes);
-            ITB_CHECK(e == cudaSuccess, "matmul_nbits: smem attribute: %s", cudaGetErrorString(e));
-            attr_smem[dev] = smem_bytes;
-        }
-    }
-    cudaLaunchConfig_t cfg{};
-    cfg.gridDim = dim3(tiles_n, splitk, 1);
-    cfg.blockDim = dim3(W4_THREADS, 1, 1);
-    cfg.dynamicSmemBytes = smem_bytes;
-    cfg.stream = st;
-    cudaLaunchAttribute attr[2];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = 1;
-    attr[0].val.clusterDim.y = splitk;
-    attr[0].val.clusterDim.z = 1;
-    attr[1].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[1].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = pdl_enabled() ? 2 : 1;
-    cudaError_t e = cudaLaunchKernelEx(&cfg, kern, grp, mapX, residual, m, k, ktiles, per, stages);
-    ITB_CHECK(e == cudaSuccess, "matmul_nbits: launch failed: %s", cudaGetErrorString(e));
-    itb::count_launch();
-    return 0;
+    return launch("matmul_nbits", gemm_skinny_w4_kernel<T, MT, BS, ZP>,
+                  {dim3(tiles_n, splitk, 1), dim3(W4_THREADS, 1, 1), smem_bytes, st, dim3(1, splitk, 1)}, grp, mapX, residual, m,
+                  k, ktiles, per, stages);
 }
 
 template <typename T, int MT, int BS>
@@ -448,14 +421,12 @@ __global__ void __launch_bounds__(256) dequant_w4_kernel(const uint8_t *__restri
 static int dequant_w4(int dtype, const void *q, const void *s, const void *zp, void *w, int k, int n, int bs, cudaStream_t st) {
     const int64_t total = (int64_t)(k / 2) * n;
     if (total == 0) return 0;
+    const LaunchCfg c{dim3(grid_for(total, 256)), dim3(256), 0, st};
     if (dtype == ITB_BF16)
-        launch_k(dequant_w4_kernel<__nv_bfloat16>, dim3(grid_for(total, 256)), dim3(256), 0, st, (const uint8_t *)q,
-                 (const __nv_bfloat16 *)s, (const uint8_t *)zp, (__nv_bfloat16 *)w, k, n, bs);
-    else
-        launch_k(dequant_w4_kernel<__half>, dim3(grid_for(total, 256)), dim3(256), 0, st, (const uint8_t *)q, (const __half *)s,
-                 (const uint8_t *)zp, (__half *)w, k, n, bs);
-    ITB_LAUNCH_CHECK("dequantize_w4");
-    return 0;
+        return launch("dequantize_w4", dequant_w4_kernel<__nv_bfloat16>, c, (const uint8_t *)q, (const __nv_bfloat16 *)s,
+                      (const uint8_t *)zp, (__nv_bfloat16 *)w, k, n, bs);
+    return launch("dequantize_w4", dequant_w4_kernel<__half>, c, (const uint8_t *)q, (const __half *)s, (const uint8_t *)zp,
+                  (__half *)w, k, n, bs);
 }
 
 // the operator contract's rules on (dtype, K, N, block size, zero points); 0 = accepted, else the error is set

@@ -387,11 +387,9 @@ extern "C" int it_b200_copy(const void *src, void *dst, int64_t bytes, void *str
     int u = pick_unit(1, {bytes}, {src, dst});
     int64_t n = bytes / u;
     UNIT_DISPATCH(u, "copy", {
-        cudaError_t e = launch_k(copy_kernel<E>, dim3(grid_for(n, 256)), dim3(256), 0, (cudaStream_t)stream,
-                                 (const E *)src, (E *)dst, n);
-        ITB_CHECK(e == cudaSuccess, "copy: %s", cudaGetErrorString(e));
+        return launch("copy", copy_kernel<E>, {dim3(grid_for(n, 256)), dim3(256), 0, (cudaStream_t)stream}, (const E *)src,
+                      (E *)dst, n);
     });
-    ITB_LAUNCH_CHECK("copy");
     return 0;
 }
 
@@ -440,10 +438,9 @@ extern "C" int it_b200_transpose(int elem_size, const void *x, void *y, int rank
         }
         int64_t L = Lb / u, units = n * elem_size / u;
         UNIT_DISPATCH(u, "transpose", {
-            launch_k(permute_rows_kernel<E>, dim3(grid_for(units, 256)), dim3(256), 0, st, (const E *)x, (E *)y, units, L, r - 1,
-                                                                       odims, istr);
+            return launch("transpose", permute_rows_kernel<E>, {dim3(grid_for(units, 256)), dim3(256), 0, st}, (const E *)x, (E *)y,
+                          units, L, r - 1, odims, istr);
         });
-        ITB_LAUNCH_CHECK("transpose");
         return 0;
     }
     // general: find q with input stride 1
@@ -463,15 +460,14 @@ extern "C" int it_b200_transpose(int elem_size, const void *x, void *y, int rank
     int64_t batch = n / (od[r - 1] * od[q]);
     int64_t blocks = tiles_j * tiles_i * batch;
     ITB_CHECK(blocks < (1ll << 31), "transpose: grid too large");
+    const LaunchCfg c{dim3((unsigned)blocks), dim3(256), 0, st};
     switch (elem_size) {
-    case 1: launch_k(permute_tiled_kernel<uint8_t>, dim3((unsigned)blocks), dim3(256), 0, st, (const uint8_t *)x, (uint8_t *)y, r, odims, istr, ostr, q, tiles_j, tiles_i); break;
-    case 2: launch_k(permute_tiled_kernel<uint16_t>, dim3((unsigned)blocks), dim3(256), 0, st, (const uint16_t *)x, (uint16_t *)y, r, odims, istr, ostr, q, tiles_j, tiles_i); break;
-    case 4: launch_k(permute_tiled_kernel<uint32_t>, dim3((unsigned)blocks), dim3(256), 0, st, (const uint32_t *)x, (uint32_t *)y, r, odims, istr, ostr, q, tiles_j, tiles_i); break;
-    case 8: launch_k(permute_tiled_kernel<uint64_t>, dim3((unsigned)blocks), dim3(256), 0, st, (const uint64_t *)x, (uint64_t *)y, r, odims, istr, ostr, q, tiles_j, tiles_i); break;
+    case 1: return launch("transpose", permute_tiled_kernel<uint8_t>, c, (const uint8_t *)x, (uint8_t *)y, r, odims, istr, ostr, q, tiles_j, tiles_i);
+    case 2: return launch("transpose", permute_tiled_kernel<uint16_t>, c, (const uint16_t *)x, (uint16_t *)y, r, odims, istr, ostr, q, tiles_j, tiles_i);
+    case 4: return launch("transpose", permute_tiled_kernel<uint32_t>, c, (const uint32_t *)x, (uint32_t *)y, r, odims, istr, ostr, q, tiles_j, tiles_i);
+    case 8: return launch("transpose", permute_tiled_kernel<uint64_t>, c, (const uint64_t *)x, (uint64_t *)y, r, odims, istr, ostr, q, tiles_j, tiles_i);
     default: ITB_FAIL("transpose: unsupported element size %d", elem_size);
     }
-    ITB_LAUNCH_CHECK("transpose");
-    return 0;
 }
 
 template <bool SPLIT>
@@ -509,9 +505,8 @@ static int concat_split_impl(const char *name, int elem_size, int n_parts, const
         if (max_n == 0) continue;
         dim3 grid(grid_for(max_n, 256, 4), cnt);
         UNIT_DISPATCH(u, name, {
-            launch_k(concat_split_kernel<E, SPLIT>, dim3(grid), dim3(256), 0, st, ps, (E *)joined, outer, Ltot);
+            if (launch(name, concat_split_kernel<E, SPLIT>, {grid, dim3(256), 0, st}, ps, (E *)joined, outer, Ltot)) return 1;
         });
-        ITB_LAUNCH_CHECK(name);
     }
     return 0;
 }
@@ -537,15 +532,14 @@ extern "C" int it_b200_gather(int elem_size, int idx_dtype, const void *data, co
     int u = pick_unit(elem_size, {inner * elem_size}, {data, out});
     int64_t inner_u = inner * elem_size / u;
     int64_t n = outer * n_idx * inner_u;
+    const LaunchCfg c{dim3(grid_for(n, 256)), dim3(256), 0, st};
     UNIT_DISPATCH(u, "gather", {
         if (idx_dtype == ITB_I64)
-            launch_k(gather_kernel<E, int64_t>, dim3(grid_for(n, 256)), dim3(256), 0, st, (const E *)data, (const int64_t *)idx,
-                                                                       (E *)out, outer, axis_len, inner_u, n_idx);
-        else
-            launch_k(gather_kernel<E, int32_t>, dim3(grid_for(n, 256)), dim3(256), 0, st, (const E *)data, (const int32_t *)idx,
-                                                                       (E *)out, outer, axis_len, inner_u, n_idx);
+            return launch("gather", gather_kernel<E, int64_t>, c, (const E *)data, (const int64_t *)idx, (E *)out, outer, axis_len,
+                          inner_u, n_idx);
+        return launch("gather", gather_kernel<E, int32_t>, c, (const E *)data, (const int32_t *)idx, (E *)out, outer, axis_len,
+                      inner_u, n_idx);
     });
-    ITB_LAUNCH_CHECK("gather");
     return 0;
 }
 
@@ -564,15 +558,14 @@ extern "C" int it_b200_pad_slice(int elem_size, const void *in, void *out, int r
     }
     if (n == 0) return 0;
     auto st = (cudaStream_t)stream;
+    const LaunchCfg c{dim3(grid_for(n, 256)), dim3(256), 0, st};
     switch (elem_size) {
-    case 1: launch_k(pad_slice_kernel<uint8_t>, dim3(grid_for(n, 256)), dim3(256), 0, st, (const uint8_t *)in, (uint8_t *)out, n, rank, din, dout, s, t); break;
-    case 2: launch_k(pad_slice_kernel<uint16_t>, dim3(grid_for(n, 256)), dim3(256), 0, st, (const uint16_t *)in, (uint16_t *)out, n, rank, din, dout, s, t); break;
-    case 4: launch_k(pad_slice_kernel<uint32_t>, dim3(grid_for(n, 256)), dim3(256), 0, st, (const uint32_t *)in, (uint32_t *)out, n, rank, din, dout, s, t); break;
-    case 8: launch_k(pad_slice_kernel<uint64_t>, dim3(grid_for(n, 256)), dim3(256), 0, st, (const uint64_t *)in, (uint64_t *)out, n, rank, din, dout, s, t); break;
+    case 1: return launch("pad_slice", pad_slice_kernel<uint8_t>, c, (const uint8_t *)in, (uint8_t *)out, n, rank, din, dout, s, t);
+    case 2: return launch("pad_slice", pad_slice_kernel<uint16_t>, c, (const uint16_t *)in, (uint16_t *)out, n, rank, din, dout, s, t);
+    case 4: return launch("pad_slice", pad_slice_kernel<uint32_t>, c, (const uint32_t *)in, (uint32_t *)out, n, rank, din, dout, s, t);
+    case 8: return launch("pad_slice", pad_slice_kernel<uint64_t>, c, (const uint64_t *)in, (uint64_t *)out, n, rank, din, dout, s, t);
     default: ITB_FAIL("pad_slice: unsupported element size %d", elem_size);
     }
-    ITB_LAUNCH_CHECK("pad_slice");
-    return 0;
 }
 
 extern "C" int it_b200_reduce(int dtype, int is_mean, const void *x, void *y, int rank, const int64_t *dims,
@@ -602,9 +595,9 @@ extern "C" int it_b200_reduce(int dtype, int is_mean, const void *x, void *y, in
     auto st = (cudaStream_t)stream;
     unsigned grid = (unsigned)((n_out * 32 + 255) / 256);
     ITB_DISPATCH_FLOAT(dtype, "reduce", {
-        launch_k(reduce_kernel<T>, dim3(grid), dim3(256), 0, st, (const T *)x, (T *)y, n_out, R, kr, kd, ks, rr, rd, rs, scale);
+        return launch("reduce", reduce_kernel<T>, {dim3(grid), dim3(256), 0, st}, (const T *)x, (T *)y, n_out, R, kr, kd, ks, rr, rd,
+                      rs, scale);
     });
-    ITB_LAUNCH_CHECK("reduce");
     return 0;
 }
 
@@ -614,9 +607,9 @@ extern "C" int it_b200_pool2d(int dtype, int is_max, const void *x, void *y, int
     int64_t n = (int64_t)N * C * OH * OW;
     if (n == 0) return 0;
     ITB_DISPATCH_FLOAT(dtype, "pool2d", {
-        launch_k(pool2d_kernel<T>, dim3(grid_for(n, 256)), dim3(256), 0, (cudaStream_t)stream, is_max, (const T *)x, (T *)y, (int64_t)N * C, H, W, kh, kw, dh, dw, ph, pw, sh, sw, OH, OW);
+        return launch("pool2d", pool2d_kernel<T>, {dim3(grid_for(n, 256)), dim3(256), 0, (cudaStream_t)stream}, is_max, (const T *)x,
+                      (T *)y, (int64_t)N * C, H, W, kh, kw, dh, dw, ph, pw, sh, sw, OH, OW);
     });
-    ITB_LAUNCH_CHECK("pool2d");
     return 0;
 }
 
@@ -628,33 +621,26 @@ extern "C" int it_b200_pool2d_nhwc(int dtype, int is_max, const void *x, void *y
     if (total == 0) return 0;
     auto st = (cudaStream_t)stream;
     if (!is_max && kh == H && kw == W && ph == 0 && pw == 0 && OH == 1 && OW == 1 && dh == 1 && dw == 1 && N <= 65535) {
-        const dim3 grid((unsigned)((C / 8 + 31) / 32), (unsigned)N);
+        const LaunchCfg c{dim3((unsigned)((C / 8 + 31) / 32), (unsigned)N), dim3(256), 0, st};
         if (dtype == ITB_F16)
-            launch_k(global_avgpool_nhwc_kernel<__half>, grid, dim3(256), 0, st, (const __half *)x, (__half *)y, C / 8, H * W);
-        else
-            launch_k(global_avgpool_nhwc_kernel<__nv_bfloat16>, grid, dim3(256), 0, st, (const __nv_bfloat16 *)x, (__nv_bfloat16 *)y, C / 8,
-                     H * W);
-        ITB_LAUNCH_CHECK("pool2d(nhwc, global average)");
-        return 0;
+            return launch("pool2d(nhwc, global average)", global_avgpool_nhwc_kernel<__half>, c, (const __half *)x, (__half *)y, C / 8,
+                          H * W);
+        return launch("pool2d(nhwc, global average)", global_avgpool_nhwc_kernel<__nv_bfloat16>, c, (const __nv_bfloat16 *)x,
+                      (__nv_bfloat16 *)y, C / 8, H * W);
     }
+    const LaunchCfg c{dim3(grid_for(total, 256)), dim3(256), 0, st};
     if (kh == 3 && kw == 3 && dh == 1 && dw == 1) {
         if (dtype == ITB_F16)
-            launch_k(pool2d_nhwc3x3_kernel<__half>, dim3(grid_for(total, 256)), dim3(256), 0, st, is_max, (const __half *)x, (__half *)y,
-                     total, C / 8, H, W, ph, pw, sh, sw, OH, OW);
-        else
-            launch_k(pool2d_nhwc3x3_kernel<__nv_bfloat16>, dim3(grid_for(total, 256)), dim3(256), 0, st, is_max, (const __nv_bfloat16 *)x,
-                     (__nv_bfloat16 *)y, total, C / 8, H, W, ph, pw, sh, sw, OH, OW);
-        ITB_LAUNCH_CHECK("pool2d(nhwc, 3x3)");
-        return 0;
+            return launch("pool2d(nhwc, 3x3)", pool2d_nhwc3x3_kernel<__half>, c, is_max, (const __half *)x, (__half *)y, total, C / 8, H,
+                          W, ph, pw, sh, sw, OH, OW);
+        return launch("pool2d(nhwc, 3x3)", pool2d_nhwc3x3_kernel<__nv_bfloat16>, c, is_max, (const __nv_bfloat16 *)x,
+                      (__nv_bfloat16 *)y, total, C / 8, H, W, ph, pw, sh, sw, OH, OW);
     }
     if (dtype == ITB_F16)
-        launch_k(pool2d_nhwc_kernel<__half>, dim3(grid_for(total, 256)), dim3(256), 0, (cudaStream_t)stream, is_max, (const __half *)x,
-                 (__half *)y, total, C / 8, H, W, kh, kw, dh, dw, ph, pw, sh, sw, OH, OW);
-    else
-        launch_k(pool2d_nhwc_kernel<__nv_bfloat16>, dim3(grid_for(total, 256)), dim3(256), 0, (cudaStream_t)stream, is_max,
-                 (const __nv_bfloat16 *)x, (__nv_bfloat16 *)y, total, C / 8, H, W, kh, kw, dh, dw, ph, pw, sh, sw, OH, OW);
-    ITB_LAUNCH_CHECK("pool2d(nhwc)");
-    return 0;
+        return launch("pool2d(nhwc)", pool2d_nhwc_kernel<__half>, c, is_max, (const __half *)x, (__half *)y, total, C / 8, H, W, kh,
+                      kw, dh, dw, ph, pw, sh, sw, OH, OW);
+    return launch("pool2d(nhwc)", pool2d_nhwc_kernel<__nv_bfloat16>, c, is_max, (const __nv_bfloat16 *)x, (__nv_bfloat16 *)y, total,
+                  C / 8, H, W, kh, kw, dh, dw, ph, pw, sh, sw, OH, OW);
 }
 
 static int batchnorm_impl(int dtype, const void *x, const float *mean, const float *var, const float *scale,
@@ -664,13 +650,11 @@ static int batchnorm_impl(int dtype, const void *x, const float *mean, const flo
     ITB_DISPATCH_FLOAT(dtype, "batchnorm", {
         constexpr int V = Vec16<T>::N;
         if (HW % V == 0 && aligned16(x) && aligned16(y))
-            launch_k(batchnorm_kernel<T, true>, dim3(grid_for(n / V, 256)), dim3(256), 0, (cudaStream_t)stream, (const T *)x,
-                     mean, var, scale, bias, (T *)y, n, C, HW, eps, relu);
-        else
-            launch_k(batchnorm_kernel<T, false>, dim3(grid_for(n, 256)), dim3(256), 0, (cudaStream_t)stream, (const T *)x,
-                     mean, var, scale, bias, (T *)y, n, C, HW, eps, relu);
+            return launch("batchnorm", batchnorm_kernel<T, true>, {dim3(grid_for(n / V, 256)), dim3(256), 0, (cudaStream_t)stream},
+                          (const T *)x, mean, var, scale, bias, (T *)y, n, C, HW, eps, relu);
+        return launch("batchnorm", batchnorm_kernel<T, false>, {dim3(grid_for(n, 256)), dim3(256), 0, (cudaStream_t)stream},
+                      (const T *)x, mean, var, scale, bias, (T *)y, n, C, HW, eps, relu);
     });
-    ITB_LAUNCH_CHECK("batchnorm");
     return 0;
 }
 

@@ -245,15 +245,14 @@ static int launch_rowop(const char *name, const T *x, T *y, const T *scale, cons
     if (outer * inner == 0 || dim == 0) return 0;
     if (inner != 1) {
         int64_t n = outer * inner;
-        launch_k(strided_kernel<T, MODE>, dim3((unsigned)((n + 255) / 256)), dim3(256), 0, st, x, y, scale, bias, outer, dim,
-                                                                           inner, scale_size, bias_size, eps);
-    } else if (dim <= 1024) {
+        return launch(name, strided_kernel<T, MODE>, {dim3((unsigned)((n + 255) / 256)), dim3(256), 0, st}, x, y, scale, bias,
+                      outer, dim, inner, scale_size, bias_size, eps);
+    }
+    if (dim <= 1024) {
         int64_t rows = outer;
-        unsigned grid = (unsigned)((rows * 32 + 255) / 256);
-#define RW(I)                                                                                  \
-    launch_k(row_warp_kernel<T, I, MODE>, dim3(grid), dim3(256), 0, st, x, y, scale, bias, rows, dim, scale_size, bias_size, eps)
-#define RWV(I)                                                                                 \
-    launch_k(row_warp_vec_kernel<T, I, MODE>, dim3(grid), dim3(256), 0, st, x, y, scale, bias, rows, dim, scale_size, bias_size, eps)
+        const LaunchCfg c{dim3((unsigned)((rows * 32 + 255) / 256)), dim3(256), 0, st};
+#define RW(I) return launch(name, row_warp_kernel<T, I, MODE>, c, x, y, scale, bias, rows, dim, scale_size, bias_size, eps)
+#define RWV(I) return launch(name, row_warp_vec_kernel<T, I, MODE>, c, x, y, scale, bias, rows, dim, scale_size, bias_size, eps)
         bool vec_ok = false;
         if constexpr (sizeof(T) == 2)
             vec_ok = dim % 8 == 0 && dim >= 64 && aligned16(x) && aligned16(y) && (!scale || scale_size != dim || aligned16(scale)) &&
@@ -274,28 +273,14 @@ static int launch_rowop(const char *name, const T *x, T *y, const T *scale, cons
         else RW(32);
 #undef RW
 #undef RWV
-    } else {
-        int cache = dim <= 12288;
-        int threads = dim >= 8192 ? 1024 : 512;
-        const size_t smem = cache ? dim * sizeof(float) : 0;
-        // a cached row of up to 12288 floats fills the 48 KB a block gets without opting in, and the kernel's static reduction
-        // buffer comes on top: rows above 48 KB - 128 B need the larger dynamic limit (per device, once)
-        if (smem > 32 * 1024) {
-            static bool raised[64] = {false};
-            int dev = 0;
-            cudaGetDevice(&dev);
-            dev &= 63;
-            if (!raised[dev]) {
-                const cudaError_t e = cudaFuncSetAttribute(row_block_kernel<T, MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                                           12288 * (int)sizeof(float));
-                ITB_CHECK(e == cudaSuccess, "%s: smem attribute: %s", name, cudaGetErrorString(e));
-                raised[dev] = true;
-            }
-        }
-        launch_k(row_block_kernel<T, MODE>, dim3((unsigned)outer), dim3(threads), smem, st, x, y, scale, bias, dim, scale_size, bias_size, eps, cache);
     }
-    ITB_LAUNCH_CHECK(name);
-    return 0;
+    // a cached row of up to 12288 floats fills the 48 KB a block gets without opting in, and the kernel's static reduction
+    // buffer comes on top: the launch raises the dynamic limit to the row
+    int cache = dim <= 12288;
+    int threads = dim >= 8192 ? 1024 : 512;
+    const int smem = cache ? dim * (int)sizeof(float) : 0;
+    return launch(name, row_block_kernel<T, MODE>, {dim3((unsigned)outer), dim3(threads), smem, st}, x, y, scale, bias, dim,
+                  scale_size, bias_size, eps, cache);
 }
 
 // ------------------------------------------------------------------ RMSNorm
@@ -455,14 +440,13 @@ static int rmsnorm_impl(int dtype, const void *x, const void *w, void *y, int64_
         int threads = hidden >= 4096 ? 512 : (hidden >= 1024 ? 256 : 128);
         const bool one = vec && hidden / Vec16<T>::N <= threads;
         auto go = [&](auto kern) {
-            launch_k(kern, dim3((unsigned)tokens), dim3(threads), 0, (cudaStream_t)stream, (const T *)x, (const T *)w, (T *)y,
-                     hidden, vec);
+            return launch("rmsnorm", kern, {dim3((unsigned)tokens), dim3(threads), 0, (cudaStream_t)stream}, (const T *)x,
+                          (const T *)w, (T *)y, hidden, vec);
         };
-        if (one && w_const) go(rmsnorm_kernel<T, true, true>);
-        else if (one) go(rmsnorm_kernel<T, true, false>);
-        else go(rmsnorm_kernel<T, false, false>);
+        if (one && w_const) return go(rmsnorm_kernel<T, true, true>);
+        if (one) return go(rmsnorm_kernel<T, true, false>);
+        return go(rmsnorm_kernel<T, false, false>);
     });
-    ITB_LAUNCH_CHECK("rmsnorm");
     return 0;
 }
 
@@ -486,24 +470,20 @@ extern "C" int it_b200_rope(int dtype, const void *pos, int pos_dtype, const voi
     if (dim_model % dim_head != 0) {
         ITB_CHECK(pos_dtype == ITB_I64 || pos_dtype == ITB_I32 || pos_dtype == ITB_U32, "rope: unsupported position dtype %d", pos_dtype);
         ITB_DISPATCH_FLOAT(dtype, "rope", {
-            int g = grid_for(rows * dim_model, 256);
+            const LaunchCfg c{dim3(grid_for(rows * dim_model, 256)), dim3(256), 0, st};
             if (pos_dtype == ITB_I64)
-                launch_k(rope_ragged_kernel<T, int64_t>, dim3(g), dim3(256), 0, st, (const int64_t *)pos, (const T *)x, (T *)y, rows, dim_model, dim_head);
-            else
-                launch_k(rope_ragged_kernel<T, int32_t>, dim3(g), dim3(256), 0, st, (const int32_t *)pos, (const T *)x, (T *)y, rows, dim_model, dim_head);
+                return launch("rope", rope_ragged_kernel<T, int64_t>, c, (const int64_t *)pos, (const T *)x, (T *)y, rows, dim_model, dim_head);
+            return launch("rope", rope_ragged_kernel<T, int32_t>, c, (const int32_t *)pos, (const T *)x, (T *)y, rows, dim_model, dim_head);
         });
-        ITB_LAUNCH_CHECK("rope");
         return 0;
     }
     ITB_DISPATCH_FLOAT(dtype, "rope", {
-        int g = grid_for(total, 256);
+        const LaunchCfg c{dim3(grid_for(total, 256)), dim3(256), 0, st};
         if (pos_dtype == ITB_I64)
-            launch_k(rope_kernel<T, int64_t>, dim3(g), dim3(256), 0, st, (const int64_t *)pos, (const T *)x, (T *)y, rows, dim_model, dim_head);
-        else if (pos_dtype == ITB_I32 || pos_dtype == ITB_U32)
-            launch_k(rope_kernel<T, int32_t>, dim3(g), dim3(256), 0, st, (const int32_t *)pos, (const T *)x, (T *)y, rows, dim_model, dim_head);
-        else
-            ITB_FAIL("rope: unsupported position dtype %d", pos_dtype);
+            return launch("rope", rope_kernel<T, int64_t>, c, (const int64_t *)pos, (const T *)x, (T *)y, rows, dim_model, dim_head);
+        if (pos_dtype == ITB_I32 || pos_dtype == ITB_U32)
+            return launch("rope", rope_kernel<T, int32_t>, c, (const int32_t *)pos, (const T *)x, (T *)y, rows, dim_model, dim_head);
+        ITB_FAIL("rope: unsupported position dtype %d", pos_dtype);
     });
-    ITB_LAUNCH_CHECK("rope");
     return 0;
 }

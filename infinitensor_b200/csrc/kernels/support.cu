@@ -1,4 +1,4 @@
-// support.cu -- error string + launch counter shared by every launcher.
+// support.cu -- error string, launch counter and shared-memory opt-ins shared by every launcher.
 #include <atomic>
 #include <cstdarg>
 #include <cstdio>
@@ -18,7 +18,26 @@ void set_error(const char *fmt, ...) {
     vsnprintf(g_err, sizeof(g_err), fmt, ap);
     va_end(ap);
 }
-void count_launch(int n) { g_launches.fetch_add(n, std::memory_order_relaxed); }
+int launched(const char *what, cudaError_t e) {
+    if (e != cudaSuccess) ITB_FAIL("%s: %s", what, cudaGetErrorString(e));
+    g_launches.fetch_add(1, std::memory_order_relaxed);
+    return 0;
+}
+// the attribute belongs to a (device, kernel) pair: a process may own runtimes on several GPUs, and every instance of a
+// kernel template is its own kernel
+int opt_in_smem(const char *what, const void *kernel, int smem) {
+    static std::mutex mu;
+    static std::map<std::pair<int, const void *>, int> granted;
+    int dev = 0;
+    cudaGetDevice(&dev);
+    std::lock_guard<std::mutex> lock(mu);
+    int &have = granted[{dev, kernel}];
+    if (smem <= have) return 0;
+    const cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+    if (e != cudaSuccess) ITB_FAIL("%s: smem attribute: %s", what, cudaGetErrorString(e));
+    have = smem;
+    return 0;
+}
 bool pdl_enabled() {
     static int v = -1;
     if (v < 0) {
