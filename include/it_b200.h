@@ -101,6 +101,12 @@ int it_b200_rmsnorm_constw(int dtype, const void *x, const void *w, void *y, int
 int it_b200_rope(int dtype, const void *pos, int pos_dtype, const void *x, void *y, int B, int S,
                  int dim_model, int dim_head, void *stream);
 
+/* ---- RoPE with a model's own frequencies: it_b200_rope, but column pair c of every head rotates by the angle
+ *      fp32(p x inv_freq[c]) (HF's inv_freq @ position_ids).  inv_freq: f32 (freq_dtype ITB_F32), at least dim_head / 2
+ *      entries; dim_model must be a multiple of dim_head. ---- */
+int it_b200_rope_freq(int dtype, const void *pos, int pos_dtype, const void *x, void *y, int B, int S, int dim_model,
+                      int dim_head, const void *inv_freq, int freq_dtype, int64_t freq_len, void *stream);
+
 /* ---- Transpose (N-d permute): replaces _transpose_kernel (transpose.cu:10-24) ---- */
 int it_b200_transpose(int elem_size, const void *x, void *y, int rank, const int64_t *dims_in,
                       const int *perm, void *stream);
@@ -353,6 +359,20 @@ int it_b200_attention_kvcache_fp8(int dtype, void *k_cache, void *v_cache, const
                                   const void *q, const void *k, const void *v, const void *position_id, int pos_flags,
                                   const void *rope_pos, int rope_pos_dtype, void *out, int B, int Hq, int Hkv, int S_max,
                                   int D, void *workspace, int64_t workspace_bytes, void *stream);
+
+/* ---- it_b200_attention_kvcache_gqa / _fp8 with the folded RoPE's angles from a table: fp32(rope_pos[b] x inv_freq[c]) for
+ *      column pair c of every head, exactly as it_b200_rope_freq.  rope_pos is required; inv_freq is f32 (freq_dtype
+ *      ITB_F32) with at least D / 2 entries, and like position_id it is read ahead of griddepcontrol.wait (a graph weight),
+ *      unless pos_flags has ITB_POS_IN_STEP. ---- */
+int it_b200_attention_kvcache_gqa_freq(int dtype, void *k_cache, void *v_cache, const void *q, const void *k, const void *v,
+                                       const void *position_id, int pos_flags, const void *rope_pos, int rope_pos_dtype,
+                                       const void *inv_freq, int freq_dtype, int64_t freq_len, void *out, int B, int Hq,
+                                       int Hkv, int S_max, int D, void *workspace, int64_t workspace_bytes, void *stream);
+int it_b200_attention_kvcache_fp8_freq(int dtype, void *k_cache, void *v_cache, const void *k_scale, const void *v_scale,
+                                       const void *q, const void *k, const void *v, const void *position_id, int pos_flags,
+                                       const void *rope_pos, int rope_pos_dtype, const void *inv_freq, int freq_dtype,
+                                       int64_t freq_len, void *out, int B, int Hq, int Hkv, int S_max, int D,
+                                       void *workspace, int64_t workspace_bytes, void *stream);
 
 /* ---- AttentionKVCache over a prompt chunk of S >= 1 new tokens (attention_prefill.cu): exactly S single-token AttentionKVCache
  *      calls in order, token i of batch row b at position p_b + i.  Caches [B,Hkv,S_max,D]; q / out [B,Hq,S,D]; k / v [B,Hkv,S,D];

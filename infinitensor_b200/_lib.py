@@ -45,6 +45,7 @@ _SIGS = {
     "it_b200_rmsnorm": (c_int, [c_int, vp, vp, vp, c_int64, c_int, vp]),
     "it_b200_rmsnorm_constw": (c_int, [c_int, vp, vp, vp, c_int64, c_int, vp]),
     "it_b200_rope": (c_int, [c_int, vp, c_int, vp, vp, c_int, c_int, c_int, c_int, vp]),
+    "it_b200_rope_freq": (c_int, [c_int, vp, c_int, vp, vp, c_int, c_int, c_int, c_int, vp, c_int, c_int64, vp]),
     "it_b200_transpose": (c_int, [c_int, vp, vp, c_int, i64p, i32p, vp]),
     "it_b200_concat": (c_int, [c_int, c_int, POINTER(vp), i64p, vp, c_int64, c_int64, vp]),
     "it_b200_split": (c_int, [c_int, c_int, POINTER(vp), i64p, vp, c_int64, c_int64, vp]),
@@ -91,6 +92,10 @@ _SIGS = {
                                               c_int, vp, c_int64, vp]),
     "it_b200_attention_kvcache_fp8": (c_int, [c_int, vp, vp, vp, vp, vp, vp, vp, vp, c_int, vp, c_int, vp, c_int, c_int, c_int,
                                               c_int, c_int, vp, c_int64, vp]),
+    "it_b200_attention_kvcache_gqa_freq": (c_int, [c_int, vp, vp, vp, vp, vp, vp, c_int, vp, c_int, vp, c_int, c_int64, vp, c_int,
+                                                   c_int, c_int, c_int, c_int, vp, c_int64, vp]),
+    "it_b200_attention_kvcache_fp8_freq": (c_int, [c_int, vp, vp, vp, vp, vp, vp, vp, vp, c_int, vp, c_int, vp, c_int, c_int64, vp,
+                                                   c_int, c_int, c_int, c_int, c_int, vp, c_int64, vp]),
     "it_b200_attention_kvcache_prompt": (c_int, [c_int, vp, vp, vp, vp, vp, vp, c_int, vp] + [c_int] * 6 + [vp]),
     "it_b200_attention_prefill": (c_int, [c_int, vp, vp, vp, vp, c_int, c_int, c_int, c_int, c_int, vp, c_int, vp, c_int64, c_int64,
                                           c_int64, c_int64, vp]),

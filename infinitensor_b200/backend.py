@@ -308,6 +308,7 @@ class GraphHandler:
     """reference GraphHandlerObj (include/core/graph_handler.h:15-159) as bound at ffi_infinitensor.cc:548-638."""
 
     head_widths = (64, 128)  # decode attention / RoPE head widths (64: extension; the reference's are 128)
+    rope_inv_freq = True  # RoPE takes the model's frequencies as an optional inv_freq input (extension)
 
     def __init__(self, runtime: CudaRuntime):
         if not isinstance(runtime, CudaRuntime):
@@ -444,9 +445,12 @@ class GraphHandler:
             ins += [k_scale, v_scale]
         return self._op1("AttentionKVCache", ins, output_matmul, [1] if per_row_positions else [])
 
-    def RoPE(self, pos, input, output, dim_head=128):
-        """dim_head (extension): rotate-half within heads of this width; the reference fixes it at 128 (rope.cc:25)."""
-        return self._op1("RoPE", [pos, input], output, [] if dim_head == 128 else [int(dim_head)])
+    def RoPE(self, pos, input, output, dim_head=128, inv_freq=None):
+        """dim_head (extension): rotate-half within heads of this width; the reference fixes it at 128 (rope.cc:25).
+        inv_freq (extension): an f32 [dim_head / 2] tensor of the model's frequencies (HF's `inv_freq` buffer, e.g.
+        `graphs.rope_inv_freq`); column pair c rotates by fp32(p * inv_freq[c]) instead of p * 10000^(-2c / dim_head)."""
+        ins = [pos, input] + ([inv_freq] if inv_freq is not None else [])
+        return self._op1("RoPE", ins, output, [] if dim_head == 128 else [int(dim_head)])
 
     def split(self, input, outputs, axis, numOrRatio):
         if isinstance(numOrRatio, int):

@@ -206,6 +206,11 @@ class RoPEB200 : public CudaKernelWithoutConfig {
         const int dim_head = 128;  // hard-coded in the reference (rope.cc:25)
 #else
         const int dim_head = as<RoPEObj>(op)->getDimHead();  // extension: 128 unless the graph gave another width
+        if (auto f = as<RoPEObj>(op)->getInvFreq()) {       // extension: the model's own frequencies
+            CK(it_b200_rope_freq(DTI(x), P(pos), DTI(pos), P(x), P(op->getOutput()), d[0], d[1], d[2], dim_head, P(f), DTI(f),
+                                 (int64_t)f->size(), S()), op);
+            return;
+        }
 #endif
         CK(it_b200_rope(DTI(x), P(pos), DTI(pos), P(x), P(op->getOutput()), d[0], d[1], d[2], dim_head, S()), op);
     }
@@ -537,7 +542,7 @@ void runSiluMul(const Operator &silu, const Operator &mul, const RuntimeObj *) {
 // position dtype + ITB_POS_* flags of an AttentionKVCache launch.  The kernel reads the position, the RoPE positions and the
 // cache rows below the position AHEAD of griddepcontrol.wait, which is only sound when a whole step separates them from their
 // writer: any of them produced by an operator of this graph (in-graph position arithmetic, Concat of the past) -> IN_STEP.
-static int attnPosFlags(const Operator &att, const Tensor &ropePos) {
+static int attnPosFlags(const Operator &att, const Tensor &ropePos, const Tensor &invFreq = nullptr) {
     auto pos = att->getInputs(5);
     int flags = DTI(pos);
     if (as<AttentionKVCacheObj>(att)->getPerRowPositions()) {
@@ -553,25 +558,42 @@ static int attnPosFlags(const Operator &att, const Tensor &ropePos) {
     }
     bool inStep = pos->getSource() != nullptr || att->getInputs(0)->getSource() != nullptr || att->getInputs(1)->getSource() != nullptr;
     if (ropePos && ropePos->getSource() != nullptr) inStep = true;
+    if (invFreq && invFreq->getSource() != nullptr) inStep = true;
     if (inStep) flags |= ITB_POS_IN_STEP;
     return flags;
 }
-// RoPE(q), RoPE(k) folded into the decode attention kernel (the aliases between them are storage no-ops)
+// RoPE(q), RoPE(k) folded into the decode attention kernel (the aliases between them are storage no-ops); the schedule folds
+// them only when they share their inv_freq table or neither has one
 void runAttentionRope(const Operator &ropeQ, const Operator &ropeK, const Operator &att, const RuntimeObj *ctx) {
     auto kc = att->getInputs(0), vc = att->getInputs(1), v = att->getInputs(4), pos = att->getInputs(5);
     auto qpre = ropeQ->getInputs(1), kpre = ropeK->getInputs(1), rpos = ropeQ->getInputs(0);
     IT_ASSERT(ropeK->getInputs(0) == rpos, "RoPE(q) and RoPE(k) must share the position tensor");
+    auto freq = as<RoPEObj>(ropeQ)->getInvFreq();
+    IT_ASSERT(as<RoPEObj>(ropeK)->getInvFreq() == freq, "RoPE(q) and RoPE(k) must share the inv_freq table");
     const auto &d = kc->getDims();
     const int hq = att->getInputs(2)->getDims()[1];  // = G x the caches' d[1] KV heads
     int64_t wsb = it_b200_attention_kvcache_workspace(d[0], hq, d[2], d[3]);
     void *ws = wsb ? RT(ctx)->getWorkspace((size_t)wsb) : nullptr;
+    const int flags = attnPosFlags(att, rpos, freq);
+    if (freq) {  // the model's own frequencies
+        const int64_t nf = (int64_t)freq->size();
+        if (as<AttentionKVCacheObj>(att)->isFp8Cache())
+            CK(it_b200_attention_kvcache_fp8_freq(DTI(qpre), P(kc), P(vc), P(att->getInputs(6)), P(att->getInputs(7)), P(qpre), P(kpre),
+                                                  P(v), P(pos), flags, P(rpos), DTI(rpos), P(freq), DTI(freq), nf, P(att->getOutput()), d[0],
+                                                  hq, d[1], d[2], d[3], ws, wsb, S()), att);
+        else
+            CK(it_b200_attention_kvcache_gqa_freq(DTI(qpre), P(kc), P(vc), P(qpre), P(kpre), P(v), P(pos), flags, P(rpos), DTI(rpos),
+                                                  P(freq), DTI(freq), nf, P(att->getOutput()), d[0], hq, d[1], d[2], d[3], ws, wsb,
+                                                  S()), att);
+        return;
+    }
     if (as<AttentionKVCacheObj>(att)->isFp8Cache()) {  // FP8 E4M3 caches + per-KV-head scales
         CK(it_b200_attention_kvcache_fp8(DTI(qpre), P(kc), P(vc), P(att->getInputs(6)), P(att->getInputs(7)), P(qpre), P(kpre), P(v),
-                                         P(pos), attnPosFlags(att, rpos), P(rpos), DTI(rpos), P(att->getOutput()), d[0], hq, d[1],
+                                         P(pos), flags, P(rpos), DTI(rpos), P(att->getOutput()), d[0], hq, d[1],
                                          d[2], d[3], ws, wsb, S()), att);
         return;
     }
-    CK(it_b200_attention_kvcache_gqa(DTI(qpre), P(kc), P(vc), P(qpre), P(kpre), P(v), P(pos), attnPosFlags(att, rpos), P(rpos),
+    CK(it_b200_attention_kvcache_gqa(DTI(qpre), P(kc), P(vc), P(qpre), P(kpre), P(v), P(pos), flags, P(rpos),
                                      DTI(rpos), P(att->getOutput()), d[0], hq, d[1], d[2], d[3], ws, wsb, S()), att);
 }
 

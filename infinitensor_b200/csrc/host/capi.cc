@@ -262,7 +262,10 @@ static Operator build_op(itb_graph *h, const string &name, const TensorVec &in, 
         return g->addOp<LayerNormObj>(in[0], in[1], o0, in.size() > 2 ? in[2] : nullptr, (float)F(0, 1e-5),
                                       (int)I(0, -1), (int)I(1, 1));
     case OpType::RMSNorm: need(2); return g->addOp<RMSNormObj>(in[0], in[1], o0);
-    case OpType::RoPE: need(2); return g->addOp<RoPEObj>(in[0], in[1], o0, (int)I(0, 128));  // iattr 0: dim_head (extension)
+    case OpType::RoPE:  // iattr 0: dim_head (extension); an optional third input: the inv_freq table (extension)
+        need(2);
+        IT_ASSERT(in.size() <= 3, "RoPE: at most 3 inputs (pos, input, inv_freq)");
+        return g->addOp<RoPEObj>(in[0], in[1], o0, (int)I(0, 128), in.size() > 2 ? in[2] : nullptr);
     case OpType::LeakyRelu: need(1); return g->addOp<LeakyReluObj>(in[0], o0, (float)F(0, 0.01));
     case OpType::Elu: need(1); return g->addOp<EluObj>(in[0], o0, (float)F(0, 1.0));
     case OpType::Relu: case OpType::Sigmoid: case OpType::Tanh: case OpType::Gelu: case OpType::Silu:

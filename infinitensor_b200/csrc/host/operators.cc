@@ -200,10 +200,17 @@ RMSNormObj::RMSNormObj(GraphObj *graph, Tensor input, Tensor weight, Tensor outp
     IT_ASSERT(checkValid(graph));
 }
 
-RoPEObj::RoPEObj(GraphObj *graph, Tensor pos, Tensor input, Tensor output, int dimHead)
-    : OperatorObj(OpType::RoPE, {pos, input}, {output}), dimHead(dimHead) {
+RoPEObj::RoPEObj(GraphObj *graph, Tensor pos, Tensor input, Tensor output, int dimHead, Tensor invFreq)
+    : OperatorObj(OpType::RoPE, invFreq ? TensorVec{pos, input, invFreq} : TensorVec{pos, input}, {output}), dimHead(dimHead) {
     IT_ASSERT(dimHead > 0 && dimHead % 2 == 0, "RoPE: dim_head " + std::to_string(dimHead) + " must be positive and even");
     IT_ASSERT(checkValid(graph));
+}
+std::optional<vector<Shape>> RoPEObj::inferShape(const TensorVec &ins) {
+    IT_ASSERT(ins.size() == 2 || ins.size() == 3, "RoPE takes 2 inputs, or 3 with an inv_freq table");
+    if (ins.size() == 3)
+        IT_ASSERT(ins[2]->getDType() == DataType::Float32 && ins[2]->getRank() == 1 && ins[2]->getDims()[0] == dimHead / 2,
+                  "RoPE: inv_freq must be f32 [dim_head / 2] = [" + std::to_string(dimHead / 2) + "]");
+    return {{ins[1]->getDims()}};
 }
 
 UnaryObj::UnaryObj(OpType type, GraphObj *graph, Tensor input, Tensor output)

@@ -133,10 +133,13 @@ class RoPEObj : public OperatorObj {
     int dimHead;  // extension: rotate-half over heads of this width; the reference fixes it at 128 (rope.cc:25)
 
   public:
-    RoPEObj(GraphObj *graph, Tensor pos, Tensor input, Tensor output, int dimHead = 128);
+    // invFreq (extension, optional): f32 [dimHead / 2]; column pair c of every head rotates by fp32(p x invFreq[c]) instead
+    // of the reference's p x 10000^(-2c / dimHead)
+    RoPEObj(GraphObj *graph, Tensor pos, Tensor input, Tensor output, int dimHead = 128, Tensor invFreq = nullptr);
     int getDimHead() const { return dimHead; }
+    Tensor getInvFreq() const { return inputs.size() > 2 ? inputs[2] : nullptr; }
     vector<int> getOpAttrVector() const override { return {(int)type.underlying(), dimHead}; }
-    std::optional<vector<Shape>> inferShape(const TensorVec &inputs) override { return {{inputs[1]->getDims()}}; }
+    std::optional<vector<Shape>> inferShape(const TensorVec &inputs) override;
     vector<DataType> inferDataType(const TensorVec &ins) const override { return {ins[1]->getDType()}; }
 };
 

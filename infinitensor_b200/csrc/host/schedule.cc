@@ -383,7 +383,8 @@ const vector<ExecStep> &GraphObj::getSchedule() {
                     if (t == op->getInputs(2)) rq = r;
                     if (t == op->getInputs(3)) rk = r;
                 }
-                if (rq && rk && rq != rk) {
+                // angles from one rule: the same inv_freq table tensor, or the base-10000 rule for both
+                if (rq && rk && rq != rk && as<RoPEObj>(rq)->getInvFreq() == as<RoPEObj>(rk)->getInvFreq()) {
                     st.kind = ExecStep::AttentionRope;
                     st.ops = {rq, rk, op};
                 } else {

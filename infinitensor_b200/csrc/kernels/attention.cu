@@ -78,6 +78,10 @@ __device__ __forceinline__ void rope_one(Vec16<T> &x, int col, const float *cs_t
     }
 }
 
+// RoPE folded into the decode attention: none, the base-10000 rule, or the angle p x inv_freq[c] from a table of the model's
+// frequencies (RoPE's optional inv_freq input, f32 [D / 2])
+enum RopeMode : int { ROPE_NONE = 0, ROPE_BASE = 1, ROPE_TABLE = 2 };
+
 // the cache holds FP8 E4M3 codes.  A namespace-scope constant: a constexpr local in the attention bodies would change how
 // their unquantised instantiations compile
 template <typename KT> constexpr bool KV8 = std::is_same_v<KT, uint8_t>;
@@ -124,13 +128,14 @@ template <typename KT> __device__ __forceinline__ auto ld_cache_row(const KT *p)
 
 constexpr int AS_MAX_B = 1024;  // batch rows whose (position, chunk count) the CTA keeps in shared memory
 
-template <typename T, typename KT, int D, int WARPS, int U, bool ROPE>
+template <typename T, typename KT, int D, int WARPS, int U, int ROPE>
 __device__ __forceinline__ void
     attn_stream_body(KT *__restrict__ kcache, KT *__restrict__ vcache, const T *__restrict__ q,
                        const T *__restrict__ kin, const T *__restrict__ vin, const void *__restrict__ position_id,
                        int pos_flags, T *__restrict__ out, int Smax, int BH, float *__restrict__ partial,
                        int slots_per_head, int *__restrict__ tickets, const void *__restrict__ rope_pos,
-                       int rope_pos_dtype, int H, const float *__restrict__ k_scale, const float *__restrict__ v_scale) {
+                       int rope_pos_dtype, int H, const float *__restrict__ k_scale, const float *__restrict__ v_scale,
+                       const float *__restrict__ inv_freq) {
     using C = RowCfg<KT, D>;
     constexpr int EPL = C::EPL, LPR = C::LPR, RPW = C::RPW;
     constexpr int VE = Vec16<T>::N, NV = EPL / VE;            // a lane's EPL activations: NV 16-byte vectors (FP8: 2)
@@ -235,14 +240,16 @@ __device__ __forceinline__ void
     }
 
     // ---------------- consumers ----------------
-    // RoPE cos / sin table of the CTA's first batch row: the RoPE positions are a step-old graph input like the cache
-    // position, so the powf / sincosf chain runs ahead of the wait; recomputed only when a later segment changes batch row
+    // RoPE cos / sin table of the CTA's first batch row: the RoPE positions (and an inv_freq table, a graph weight) are
+    // step-old like the cache position, so the powf / sincosf chain runs ahead of the wait; recomputed only when a later
+    // segment changes batch row
     int table_b = -1;
     auto rope_table = [&](int b) {
         if (threadIdx.x < D / 2) {
             const float p = rope_pos_dtype == ITB_I64 ? (float)(int)((const int64_t *)rope_pos)[b]
                                                       : (float)((const int32_t *)rope_pos)[b];
-            const float freq = p * powf(10000.f, -(float)(threadIdx.x * 2) / (float)D);
+            const float freq = ROPE == ROPE_TABLE ? __fmul_rn(p, inv_freq[threadIdx.x])
+                                                  : p * powf(10000.f, -(float)(threadIdx.x * 2) / (float)D);
             s_cs[threadIdx.x] = round_t<T>(cosf(freq));
             s_sn[threadIdx.x] = round_t<T>(sinf(freq));
         }
@@ -527,13 +534,13 @@ template <typename T, int D, typename KT = T> struct GqaCfg {  // KT: the cache 
     static constexpr int PLD = CH + 16 / (int)sizeof(T);
 };
 
-template <typename T, typename KT, int D, int QT, bool ROPE, typename... Scale>
+template <typename T, typename KT, int D, int QT, int ROPE, typename... Scale>
 __device__ __forceinline__ void
     attn_gqa_body(KT *__restrict__ kcache, KT *__restrict__ vcache, const T *__restrict__ q,
                     const T *__restrict__ kin, const T *__restrict__ vin, const void *__restrict__ position_id,
                     int pos_flags, T *__restrict__ out, int Smax, int Bn, int Hkv, int G, int NQG,
                     float *__restrict__ partial, int slots_per_head, int *__restrict__ tickets, const void *__restrict__ rope_pos, int rope_pos_dtype,
-                    const Scale *__restrict__... kv_scale) {
+                    const float *__restrict__ inv_freq, const Scale *__restrict__... kv_scale) {
     // kv_scale: k_scale, v_scale for an FP8 cache, nothing for the others (unused scale parameters alone change how the
     // unquantised kernels compile)
     using C = RowCfg<T, D>;  // row-load layout of q and the appended k / v
@@ -648,7 +655,8 @@ __device__ __forceinline__ void
         if (threadIdx.x < D / 2) {
             const float p = rope_pos_dtype == ITB_I64 ? (float)(int)((const int64_t *)rope_pos)[b]
                                                       : (float)((const int32_t *)rope_pos)[b];
-            const float freq = p * powf(10000.f, -(float)(threadIdx.x * 2) / (float)D);
+            const float freq = ROPE == ROPE_TABLE ? __fmul_rn(p, inv_freq[threadIdx.x])
+                                                  : p * powf(10000.f, -(float)(threadIdx.x * 2) / (float)D);
             s_cs[threadIdx.x] = round_t<T>(cosf(freq));
             s_sn[threadIdx.x] = round_t<T>(sinf(freq));
         }
@@ -1088,31 +1096,46 @@ __device__ __forceinline__ void
 
 template <typename T, int WARPS, int U, bool ROPE>
 __global__ void __launch_bounds__((WARPS + 1) * 32, AS_CTAS_PER_SM) attn_stream_kernel(ITB_ATTN_STREAM_ARGS(T)) {
-    attn_stream_body<T, T, 128, WARPS, U, ROPE>(ITB_ATTN_STREAM_PASS, nullptr, nullptr);  // (pdl_trigger / pdl_wait inside)
+    attn_stream_body<T, T, 128, WARPS, U, ROPE ? ROPE_BASE : ROPE_NONE>(ITB_ATTN_STREAM_PASS, nullptr, nullptr, nullptr);  // (pdl_trigger / pdl_wait inside)
 }
 template <typename T, int WARPS, int U, bool ROPE>
 __global__ void __launch_bounds__((WARPS + 1) * 32, AS_CTAS_PER_SM) attn_stream64_kernel(ITB_ATTN_STREAM_ARGS(T)) {
-    attn_stream_body<T, T, 64, WARPS, U, ROPE>(ITB_ATTN_STREAM_PASS, nullptr, nullptr);  // (pdl_trigger / pdl_wait inside)
+    attn_stream_body<T, T, 64, WARPS, U, ROPE ? ROPE_BASE : ROPE_NONE>(ITB_ATTN_STREAM_PASS, nullptr, nullptr, nullptr);  // (pdl_trigger / pdl_wait inside)
 }
 template <typename T, int QT, bool ROPE>
 __global__ void __launch_bounds__((GQ_WARPS + 1) * 32, AS_CTAS_PER_SM) attn_gqa_kernel(ITB_ATTN_GQA_ARGS(T)) {
-    attn_gqa_body<T, T, 128, QT, ROPE>(ITB_ATTN_GQA_PASS);  // (pdl_trigger / pdl_wait inside)
+    attn_gqa_body<T, T, 128, QT, ROPE ? ROPE_BASE : ROPE_NONE>(ITB_ATTN_GQA_PASS, nullptr);  // (pdl_trigger / pdl_wait inside)
 }
 template <typename T, int QT, bool ROPE>
 __global__ void __launch_bounds__((GQ_WARPS + 1) * 32, AS_CTAS_PER_SM) attn_gqa64_kernel(ITB_ATTN_GQA_ARGS(T)) {
-    attn_gqa_body<T, T, 64, QT, ROPE>(ITB_ATTN_GQA_PASS);  // (pdl_trigger / pdl_wait inside)
+    attn_gqa_body<T, T, 64, QT, ROPE ? ROPE_BASE : ROPE_NONE>(ITB_ATTN_GQA_PASS, nullptr);  // (pdl_trigger / pdl_wait inside)
 }
 
 // FP8 E4M3 caches: uint8_t codes + one fp32 scale per KV head, f16 / bf16 activations, both widths in one name each
 template <typename T, int D, int WARPS, int U, bool ROPE>
 __global__ void __launch_bounds__((WARPS + 1) * 32, AS_CTAS_PER_SM)
     attn_stream_kv8_kernel(ITB_ATTN_STREAM_ARGS(uint8_t), const float *__restrict__ k_scale, const float *__restrict__ v_scale) {
-    attn_stream_body<T, uint8_t, D, WARPS, U, ROPE>(ITB_ATTN_STREAM_PASS, k_scale, v_scale);  // (pdl_trigger / pdl_wait inside)
+    attn_stream_body<T, uint8_t, D, WARPS, U, ROPE ? ROPE_BASE : ROPE_NONE>(ITB_ATTN_STREAM_PASS, k_scale, v_scale, nullptr);  // (pdl_trigger / pdl_wait inside)
 }
 template <typename T, int D, int QT, bool ROPE>
 __global__ void __launch_bounds__((GQ_WARPS + 1) * 32, AS_CTAS_PER_SM)
     attn_gqa_kv8_kernel(ITB_ATTN_GQA_ARGS(uint8_t), const float *__restrict__ k_scale, const float *__restrict__ v_scale) {
-    attn_gqa_body<T, uint8_t, D, QT, ROPE>(ITB_ATTN_GQA_PASS, k_scale, v_scale);  // (pdl_trigger / pdl_wait inside)
+    attn_gqa_body<T, uint8_t, D, QT, ROPE ? ROPE_BASE : ROPE_NONE>(ITB_ATTN_GQA_PASS, nullptr, k_scale, v_scale);  // (pdl_trigger / pdl_wait inside)
+}
+
+// RoPE from an inv_freq table: one name per body for every cache type and width (k_scale / v_scale: FP8 caches only)
+template <typename T, typename KT, int D, int WARPS, int U>
+__global__ void __launch_bounds__((WARPS + 1) * 32, AS_CTAS_PER_SM)
+    attn_stream_freq_kernel(ITB_ATTN_STREAM_ARGS(KT), const float *__restrict__ inv_freq, const float *__restrict__ k_scale,
+                            const float *__restrict__ v_scale) {
+    attn_stream_body<T, KT, D, WARPS, U, ROPE_TABLE>(ITB_ATTN_STREAM_PASS, k_scale, v_scale, inv_freq);  // (pdl_trigger / pdl_wait inside)
+}
+template <typename T, typename KT, int D, int QT>
+__global__ void __launch_bounds__((GQ_WARPS + 1) * 32, AS_CTAS_PER_SM)
+    attn_gqa_freq_kernel(ITB_ATTN_GQA_ARGS(KT), const float *__restrict__ inv_freq, const float *__restrict__ k_scale,
+                         const float *__restrict__ v_scale) {
+    if constexpr (KV8<KT>) attn_gqa_body<T, KT, D, QT, ROPE_TABLE>(ITB_ATTN_GQA_PASS, inv_freq, k_scale, v_scale);
+    else attn_gqa_body<T, KT, D, QT, ROPE_TABLE>(ITB_ATTN_GQA_PASS, inv_freq);  // (pdl_trigger / pdl_wait inside)
 }
 
 }  // namespace itb
@@ -1125,9 +1148,9 @@ extern "C" int64_t it_b200_attention_kvcache_workspace(int B, int H, int S_max, 
     return (int64_t)B * H * stream_slots_per_head(S_max) * (D + 2) * sizeof(float);
 }
 
-template <typename T, typename KT, int D, bool ROPE>
+template <typename T, typename KT, int D, int ROPE>
 static int launch_attn_stream(KT *kc, KT *vc, const T *q, const T *k, const T *v, const void *position_id, int pos_flags,
-                              const void *rope_pos, int rope_pos_dtype, T *out, int BH, int H, int S_max,
+                              const void *rope_pos, int rope_pos_dtype, const float *inv_freq, T *out, int BH, int H, int S_max,
                               float *workspace, const float *k_scale, const float *v_scale, cudaStream_t st) {
     constexpr int WARPS = 8, U = 4;  // consumer warps x rows per lane and chunk
     constexpr int CH = WARPS * RowCfg<KT, D>::RPW * U;
@@ -1137,17 +1160,19 @@ static int launch_attn_stream(KT *kc, KT *vc, const T *q, const T *k, const T *v
     if (!tickets) ITB_FAIL("%s: no ticket pool", what);
     const int64_t max_units = (int64_t)BH * (S_max / CH + 1);
     const int grid = (int)std::min<int64_t>(max_units, (int64_t)AS_CTAS_PER_SM * kNumSMs);
-    auto go = [&](auto kern, auto... scales) {  // scales: FP8 only
+    auto go = [&](auto kern, auto... extra) {  // extra: the inv_freq table, FP8 scales
         return launch(what, kern, {dim3(grid), dim3((WARPS + 1) * 32), smem, st}, kc, vc, q, k, v, position_id, pos_flags, out,
-                      S_max, BH, workspace, stream_slots_per_head(S_max), tickets, rope_pos, rope_pos_dtype, H, scales...);
+                      S_max, BH, workspace, stream_slots_per_head(S_max), tickets, rope_pos, rope_pos_dtype, H, extra...);
     };
-    if constexpr (std::is_same_v<KT, uint8_t>) return go(attn_stream_kv8_kernel<T, D, WARPS, U, ROPE>, k_scale, v_scale);
-    else return go(D == 128 ? attn_stream_kernel<T, WARPS, U, ROPE> : attn_stream64_kernel<T, WARPS, U, ROPE>);
+    constexpr bool R = ROPE == ROPE_BASE;
+    if constexpr (ROPE == ROPE_TABLE) return go(attn_stream_freq_kernel<T, KT, D, WARPS, U>, inv_freq, k_scale, v_scale);
+    else if constexpr (std::is_same_v<KT, uint8_t>) return go(attn_stream_kv8_kernel<T, D, WARPS, U, R>, k_scale, v_scale);
+    else return go(D == 128 ? attn_stream_kernel<T, WARPS, U, R> : attn_stream64_kernel<T, WARPS, U, R>);
 }
 
-template <typename T, typename KT, int D, int QT, bool ROPE>
+template <typename T, typename KT, int D, int QT, int ROPE>
 static int launch_attn_gqa(KT *kc, KT *vc, const T *q, const T *k, const T *v, const void *position_id, int pos_flags,
-                           const void *rope_pos, int rope_pos_dtype, T *out, int B, int Hkv, int G, int S_max,
+                           const void *rope_pos, int rope_pos_dtype, const float *inv_freq, T *out, int B, int Hkv, int G, int S_max,
                            float *workspace, const float *k_scale, const float *v_scale, cudaStream_t st) {
     constexpr int CH = GqaCfg<T, D, KT>::CH;
     constexpr int smem = AS_STAGES * 2 * CH * D * (int)sizeof(KT);
@@ -1157,44 +1182,50 @@ static int launch_attn_gqa(KT *kc, KT *vc, const T *q, const T *k, const T *v, c
     if (!tickets) ITB_FAIL("%s: no ticket pool", what);
     const int64_t max_units = (int64_t)B * Hkv * nqg * (S_max / CH + 1);
     const int grid = (int)std::min<int64_t>(max_units, (int64_t)AS_CTAS_PER_SM * kNumSMs);
-    auto go = [&](auto kern, auto... scales) {  // scales: FP8 only
+    auto go = [&](auto kern, auto... extra) {  // extra: the inv_freq table, FP8 scales
         return launch(what, kern, {dim3(grid), dim3((GQ_WARPS + 1) * 32), smem, st}, kc, vc, q, k, v, position_id, pos_flags,
                       out, S_max, B, Hkv, G, nqg, workspace, stream_slots_per_head(S_max), tickets, rope_pos, rope_pos_dtype,
-                      scales...);
+                      extra...);
     };
-    if constexpr (std::is_same_v<KT, uint8_t>) return go(attn_gqa_kv8_kernel<T, D, QT, ROPE>, k_scale, v_scale);
-    else return go(D == 128 ? attn_gqa_kernel<T, QT, ROPE> : attn_gqa64_kernel<T, QT, ROPE>);
+    constexpr bool R = ROPE == ROPE_BASE;
+    if constexpr (ROPE == ROPE_TABLE) return go(attn_gqa_freq_kernel<T, KT, D, QT>, inv_freq, k_scale, v_scale);
+    else if constexpr (std::is_same_v<KT, uint8_t>) return go(attn_gqa_kv8_kernel<T, D, QT, R>, k_scale, v_scale);
+    else return go(D == 128 ? attn_gqa_kernel<T, QT, R> : attn_gqa64_kernel<T, QT, R>);
 }
 
-// the kernel for head width D and G = Hq / Hkv, with RoPE folded in when rope_pos is given.  G > 1 takes one query tile of
-// 16 rows for G <= 16, else groups of two tiles (four tiles spill registers and, for fp32, exceed the static shared memory)
+// the kernel for head width D and G = Hq / Hkv, with RoPE folded in when rope_pos is given (angles from inv_freq when that
+// is given too).  G > 1 takes one query tile of 16 rows for G <= 16, else groups of two tiles (four tiles spill registers
+// and, for fp32, exceed the static shared memory)
 template <typename T, typename KT, int D>
 static int launch_attn_width(KT *kc, KT *vc, const T *q, const T *k, const T *v, const void *position_id, int pos_flags,
-                             const void *rope_pos, int rope_pos_dtype, T *out, int B, int Hq, int Hkv, int S_max,
-                             float *workspace, const float *k_scale, const float *v_scale, cudaStream_t st) {
+                             const void *rope_pos, int rope_pos_dtype, const float *inv_freq, T *out, int B, int Hq, int Hkv,
+                             int S_max, float *workspace, const float *k_scale, const float *v_scale, cudaStream_t st) {
     const int G = Hq / Hkv;
     auto go = [&](auto rope) {
-        constexpr bool R = decltype(rope)::value;
+        constexpr int R = decltype(rope)::value;
         const void *rp = R ? rope_pos : nullptr;
         const int rpd = R ? rope_pos_dtype : 0;
         if (G == 1)
-            return launch_attn_stream<T, KT, D, R>(kc, vc, q, k, v, position_id, pos_flags, rp, rpd, out, B * Hq, Hq, S_max,
-                                                   workspace, k_scale, v_scale, st);
+            return launch_attn_stream<T, KT, D, R>(kc, vc, q, k, v, position_id, pos_flags, rp, rpd, inv_freq, out, B * Hq, Hq,
+                                                   S_max, workspace, k_scale, v_scale, st);
         if (G <= 16)
-            return launch_attn_gqa<T, KT, D, 1, R>(kc, vc, q, k, v, position_id, pos_flags, rp, rpd, out, B, Hkv, G, S_max,
-                                                   workspace, k_scale, v_scale, st);
-        return launch_attn_gqa<T, KT, D, 2, R>(kc, vc, q, k, v, position_id, pos_flags, rp, rpd, out, B, Hkv, G, S_max,
+            return launch_attn_gqa<T, KT, D, 1, R>(kc, vc, q, k, v, position_id, pos_flags, rp, rpd, inv_freq, out, B, Hkv, G,
+                                                   S_max, workspace, k_scale, v_scale, st);
+        return launch_attn_gqa<T, KT, D, 2, R>(kc, vc, q, k, v, position_id, pos_flags, rp, rpd, inv_freq, out, B, Hkv, G, S_max,
                                                workspace, k_scale, v_scale, st);
     };
-    return rope_pos ? go(std::true_type{}) : go(std::false_type{});
+    if (!rope_pos) return go(std::integral_constant<int, ROPE_NONE>{});
+    return inv_freq ? go(std::integral_constant<int, ROPE_TABLE>{}) : go(std::integral_constant<int, ROPE_BASE>{});
 }
 
 // Hq query heads over Hkv cache heads.  Hq == Hkv runs attn_stream_kernel; Hq = G Hkv, G > 1, runs attn_gqa_kernel.
 // k_scale non-null: the caches hold FP8 E4M3 codes (attn_*_kv8_kernel).
+// inv_freq non-null: the folded RoPE's angles are p x inv_freq[c] (f32 [D / 2], checked by the caller).
 static int attention_impl(int dtype, void *k_cache, void *v_cache, const void *q, const void *k, const void *v,
                           const void *position_id, int pos_flags, const void *rope_pos, int rope_pos_dtype, void *out,
                           int B, int Hq, int Hkv, int S_max, int D, void *workspace, int64_t workspace_bytes,
-                          void *stream, const float *k_scale = nullptr, const float *v_scale = nullptr) {
+                          void *stream, const float *k_scale = nullptr, const float *v_scale = nullptr,
+                          const float *inv_freq = nullptr) {
     const int H = Hq;
     const int pos_dtype = pos_flags & 0xff;
     // 128: the reference's only width (attention_kvcache.cu:154); 64: GPT-2 / TinyLlama heads (extension)
@@ -1223,14 +1254,14 @@ static int attention_impl(int dtype, void *k_cache, void *v_cache, const void *q
             using T = decltype(tag);
             auto go = D == 64 ? launch_attn_width<T, uint8_t, 64> : launch_attn_width<T, uint8_t, 128>;
             return go((uint8_t *)k_cache, (uint8_t *)v_cache, (const T *)q, (const T *)k, (const T *)v, position_id, pos_flags,
-                      rope_pos, rope_pos_dtype, (T *)out, B, Hq, Hkv, S_max, (float *)workspace, k_scale, v_scale, st);
+                      rope_pos, rope_pos_dtype, inv_freq, (T *)out, B, Hq, Hkv, S_max, (float *)workspace, k_scale, v_scale, st);
         };
         return dtype == ITB_F16 ? fp8(__half{}) : fp8(__nv_bfloat16{});
     }
     ITB_DISPATCH_FLOAT(dtype, "AttentionKVCache", {
         auto go = D == 64 ? launch_attn_width<T, T, 64> : launch_attn_width<T, T, 128>;
         return go((T *)k_cache, (T *)v_cache, (const T *)q, (const T *)k, (const T *)v, position_id, pos_flags, rope_pos,
-                  rope_pos_dtype, (T *)out, B, Hq, Hkv, S_max, (float *)workspace, nullptr, nullptr, st);
+                  rope_pos_dtype, inv_freq, (T *)out, B, Hq, Hkv, S_max, (float *)workspace, nullptr, nullptr, st);
     });
     return 0;
 }
@@ -1267,4 +1298,37 @@ extern "C" int it_b200_attention_kvcache_fp8(int dtype, void *k_cache, void *v_c
     ITB_CHECK(k_scale && v_scale, "AttentionKVCache(FP8 cache): k_scale and v_scale are required");
     return attention_impl(dtype, k_cache, v_cache, q, k, v, position_id, pos_flags, rope_pos, rope_pos_dtype, out, B, Hq, Hkv,
                           S_max, D, workspace, workspace_bytes, stream, (const float *)k_scale, (const float *)v_scale);
+}
+
+// a RoPE inv_freq table: f32, at least D / 2 entries, 4-byte aligned, and only with RoPE positions
+static int check_inv_freq(const char *what, const void *rope_pos, const void *inv_freq, int freq_dtype, int64_t freq_len, int D) {
+    ITB_CHECK(inv_freq, "%s: inv_freq table missing", what);
+    ITB_CHECK(rope_pos, "%s: an inv_freq table needs RoPE positions", what);
+    ITB_CHECK(freq_dtype == ITB_F32, "%s: inv_freq must be f32 (dtype %d)", what, freq_dtype);
+    ITB_CHECK(freq_len >= D / 2, "%s: inv_freq has %lld entries, dim_head %d needs %d", what, (long long)freq_len, D, D / 2);
+    ITB_CHECK((reinterpret_cast<uintptr_t>(inv_freq) & 3) == 0, "%s: inv_freq must be 4-byte aligned", what);
+    return 0;
+}
+
+extern "C" int it_b200_attention_kvcache_gqa_freq(int dtype, void *k_cache, void *v_cache, const void *q, const void *k,
+                                                  const void *v, const void *position_id, int pos_flags, const void *rope_pos,
+                                                  int rope_pos_dtype, const void *inv_freq, int freq_dtype, int64_t freq_len,
+                                                  void *out, int B, int Hq, int Hkv, int S_max, int D, void *workspace,
+                                                  int64_t workspace_bytes, void *stream) {
+    if (check_inv_freq("AttentionKVCache+RoPE", rope_pos, inv_freq, freq_dtype, freq_len, D)) return 1;
+    return attention_impl(dtype, k_cache, v_cache, q, k, v, position_id, pos_flags, rope_pos, rope_pos_dtype, out, B, Hq,
+                          Hkv, S_max, D, workspace, workspace_bytes, stream, nullptr, nullptr, (const float *)inv_freq);
+}
+
+extern "C" int it_b200_attention_kvcache_fp8_freq(int dtype, void *k_cache, void *v_cache, const void *k_scale,
+                                                  const void *v_scale, const void *q, const void *k, const void *v,
+                                                  const void *position_id, int pos_flags, const void *rope_pos,
+                                                  int rope_pos_dtype, const void *inv_freq, int freq_dtype, int64_t freq_len,
+                                                  void *out, int B, int Hq, int Hkv, int S_max, int D, void *workspace,
+                                                  int64_t workspace_bytes, void *stream) {
+    ITB_CHECK(k_scale && v_scale, "AttentionKVCache(FP8 cache): k_scale and v_scale are required");
+    if (check_inv_freq("AttentionKVCache(FP8 cache)+RoPE", rope_pos, inv_freq, freq_dtype, freq_len, D)) return 1;
+    return attention_impl(dtype, k_cache, v_cache, q, k, v, position_id, pos_flags, rope_pos, rope_pos_dtype, out, B, Hq, Hkv,
+                          S_max, D, workspace, workspace_bytes, stream, (const float *)k_scale, (const float *)v_scale,
+                          (const float *)inv_freq);
 }

@@ -352,10 +352,10 @@ __global__ void __launch_bounds__(512) rmsnorm_kernel(const T *__restrict__ x, c
 }
 
 // ------------------------------------------------------------------ RoPE (rotate-half)
-template <typename T, typename P>
-__global__ void __launch_bounds__(256) rope_kernel(const P *__restrict__ pos, const T *__restrict__ x,
-                                                   T *__restrict__ y, int64_t rows, int dim_model,
-                                                   int dim_head) {
+// column pair c of a head rotates by p x 10000^(-2c / dim_head), or with an inv_freq table (TABLE) by fp32(p x inv_freq[c])
+template <typename T, typename P, bool TABLE>
+__device__ __forceinline__ void rope_body(const P *__restrict__ pos, const T *__restrict__ x, T *__restrict__ y, int64_t rows,
+                                          int dim_model, int dim_head, const float *__restrict__ inv_freq) {
     pdl_trigger();
     pdl_wait();
     int half = dim_head >> 1;
@@ -368,7 +368,7 @@ __global__ void __launch_bounds__(256) rope_kernel(const P *__restrict__ pos, co
         int head = pr / half, c = pr - head * half;
         int lo = head * dim_head + c, hi = lo + half;
         float p = (float)(int)pos[row];
-        float freq = p * powf(10000.f, -(float)(c * 2) / (float)dim_head);
+        float freq = TABLE ? __fmul_rn(p, inv_freq[c]) : p * powf(10000.f, -(float)(c * 2) / (float)dim_head);
         float cs = round_t<T>(cosf(freq)), sn = round_t<T>(sinf(freq));
         float xl = to_f(x[row * dim_model + lo]), xh = to_f(x[row * dim_model + hi]);
         // arithmetic in T exactly as rope.cu:21-29: each product and the sum rounded to T (__fmul_rn: for fp32 the compiler must
@@ -378,6 +378,18 @@ __global__ void __launch_bounds__(256) rope_kernel(const P *__restrict__ pos, co
         y[row * dim_model + lo] = from_f<T>(ol);
         y[row * dim_model + hi] = from_f<T>(oh);
     }
+}
+template <typename T, typename P>
+__global__ void __launch_bounds__(256) rope_kernel(const P *__restrict__ pos, const T *__restrict__ x,
+                                                   T *__restrict__ y, int64_t rows, int dim_model,
+                                                   int dim_head) {
+    rope_body<T, P, false>(pos, x, y, rows, dim_model, dim_head, nullptr);  // (pdl_trigger / pdl_wait inside)
+}
+template <typename T, typename P>
+__global__ void __launch_bounds__(256) rope_freq_kernel(const P *__restrict__ pos, const T *__restrict__ x, T *__restrict__ y,
+                                                        int64_t rows, int dim_model, int dim_head,
+                                                        const float *__restrict__ inv_freq) {
+    rope_body<T, P, true>(pos, x, y, rows, dim_model, dim_head, inv_freq);  // (pdl_trigger / pdl_wait inside)
 }
 
 // dim_model not a multiple of dim_head (the reference's own golden test runs dim_model = 32 against its hard-coded 128-wide
@@ -460,14 +472,15 @@ extern "C" int it_b200_rmsnorm_constw(int dtype, const void *x, const void *w, v
     return rmsnorm_impl(dtype, x, w, y, tokens, hidden, true, stream);
 }
 
-extern "C" int it_b200_rope(int dtype, const void *pos, int pos_dtype, const void *x, void *y, int B, int S,
-                            int dim_model, int dim_head, void *stream) {
+static int rope_impl(int dtype, const void *pos, int pos_dtype, const void *x, void *y, int B, int S, int dim_model,
+                     int dim_head, const float *inv_freq, void *stream) {
     ITB_CHECK(dim_head > 0 && dim_head % 2 == 0, "rope: dim_head %d must be even", dim_head);
     int64_t rows = (int64_t)B * S;
     if (rows == 0) return 0;
     int64_t total = rows * (dim_model / 2);
     auto st = (cudaStream_t)stream;
     if (dim_model % dim_head != 0) {
+        ITB_CHECK(!inv_freq, "rope: an inv_freq table needs dim_model (%d) to be a multiple of dim_head (%d)", dim_model, dim_head);
         ITB_CHECK(pos_dtype == ITB_I64 || pos_dtype == ITB_I32 || pos_dtype == ITB_U32, "rope: unsupported position dtype %d", pos_dtype);
         ITB_DISPATCH_FLOAT(dtype, "rope", {
             const LaunchCfg c{dim3(grid_for(rows * dim_model, 256)), dim3(256), 0, st};
@@ -479,11 +492,31 @@ extern "C" int it_b200_rope(int dtype, const void *pos, int pos_dtype, const voi
     }
     ITB_DISPATCH_FLOAT(dtype, "rope", {
         const LaunchCfg c{dim3(grid_for(total, 256)), dim3(256), 0, st};
-        if (pos_dtype == ITB_I64)
+        const bool p64 = pos_dtype == ITB_I64;
+        if (!p64 && pos_dtype != ITB_I32 && pos_dtype != ITB_U32) ITB_FAIL("rope: unsupported position dtype %d", pos_dtype);
+        if (inv_freq) {
+            if (p64) return launch("rope", rope_freq_kernel<T, int64_t>, c, (const int64_t *)pos, (const T *)x, (T *)y, rows, dim_model, dim_head, inv_freq);
+            return launch("rope", rope_freq_kernel<T, int32_t>, c, (const int32_t *)pos, (const T *)x, (T *)y, rows, dim_model, dim_head, inv_freq);
+        }
+        if (p64)
             return launch("rope", rope_kernel<T, int64_t>, c, (const int64_t *)pos, (const T *)x, (T *)y, rows, dim_model, dim_head);
-        if (pos_dtype == ITB_I32 || pos_dtype == ITB_U32)
-            return launch("rope", rope_kernel<T, int32_t>, c, (const int32_t *)pos, (const T *)x, (T *)y, rows, dim_model, dim_head);
-        ITB_FAIL("rope: unsupported position dtype %d", pos_dtype);
+        return launch("rope", rope_kernel<T, int32_t>, c, (const int32_t *)pos, (const T *)x, (T *)y, rows, dim_model, dim_head);
     });
     return 0;
+}
+
+extern "C" int it_b200_rope(int dtype, const void *pos, int pos_dtype, const void *x, void *y, int B, int S,
+                            int dim_model, int dim_head, void *stream) {
+    return rope_impl(dtype, pos, pos_dtype, x, y, B, S, dim_model, dim_head, nullptr, stream);
+}
+
+extern "C" int it_b200_rope_freq(int dtype, const void *pos, int pos_dtype, const void *x, void *y, int B, int S,
+                                 int dim_model, int dim_head, const void *inv_freq, int freq_dtype, int64_t freq_len,
+                                 void *stream) {
+    ITB_CHECK(inv_freq, "rope: inv_freq table missing");
+    ITB_CHECK(freq_dtype == ITB_F32, "rope: inv_freq must be f32 (dtype %d)", freq_dtype);
+    ITB_CHECK(dim_head > 0 && freq_len >= dim_head / 2, "rope: inv_freq has %lld entries, dim_head %d needs %d",
+              (long long)freq_len, dim_head, dim_head / 2);
+    ITB_CHECK((reinterpret_cast<uintptr_t>(inv_freq) & 3) == 0, "rope: inv_freq must be 4-byte aligned");
+    return rope_impl(dtype, pos, pos_dtype, x, y, B, S, dim_model, dim_head, (const float *)inv_freq, stream);
 }

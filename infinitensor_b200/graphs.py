@@ -4,7 +4,9 @@ need no `onnx` package.  Every builder takes a duck-typed handler: `backend.Grap
 or `oracle.graph_oracle.OracleHandler` (the CPU checker) -- one graph description, two executors.  Decode graphs with
 attention heads narrower than 128 (GPT-2, TinyLlama) use an extension of the reference, whose AttentionKVCache scale and
 RoPE are fixed at 128: they build only on a handler that lists the width in its `head_widths` (`GraphHandler` does;
-`OracleHandler`, which restates the reference, does not), so no executor quietly applies the 128-wide rule to them.
+`OracleHandler`, which restates the reference, does not), so no executor quietly applies the 128-wide rule to them.  Likewise
+a Llama config with other RoPE frequencies than base 10000 (`rope_theta`, `rope_scaling`) builds only on a handler whose
+RoPE takes an inv_freq table (`rope_inv_freq`).
 
   build_llama_decode   -- config C3/C5: Llama-7B-shape KV-cache decode step (op mix of
                           examples/python/llama_kvcache_inference.py:45-80 with fused RMSNorm / RoPE /
@@ -63,7 +65,42 @@ def _require_head_width(h, dh: int):
         raise NotImplementedError(f"{type(h).__name__} does not execute {dh}-wide attention heads (the reference's are 128-wide)")
 
 
+def _require_rope_table(h, cfg):
+    if not getattr(h, "rope_inv_freq", False):
+        raise NotImplementedError(f"{type(h).__name__} has no RoPE inv_freq table: it cannot run rope_theta = {cfg.rope_theta}, "
+                                  f"rope_scaling = {cfg.rope_scaling} (its RoPE is base 10000)")
+
+
+def rope_inv_freq(dim_head: int, theta: float = 10000.0, scaling: dict | None = None) -> np.ndarray:
+    """RoPE's inv_freq table, f32 [dim_head / 2], as Hugging Face transformers computes it in float32: the default rule
+    1 / theta^(2c / dim_head), and with scaling {"type": "llama3", factor, low_freq_factor, high_freq_factor,
+    original_max_position_embeddings} Llama-3.1's rule: columns whose wavelength 2 pi / inv_freq is below
+    original / high_freq_factor keep their frequency, those above original / low_freq_factor are divided by factor, and the
+    band between is interpolated.  Rope types that also scale attention (YaRN, LongRoPE) and dynamic NTK are not covered."""
+    f32 = np.float32
+    expo = np.arange(0, dim_head, 2, dtype=np.int64).astype(f32) / f32(dim_head)
+    inv = f32(1.0) / np.power(np.float64(f32(theta)), expo.astype(np.float64)).astype(f32)  # (a correctly rounded f32 power)
+    if scaling is None:
+        return inv.astype(f32)
+    kind = scaling.get("type", scaling.get("rope_type"))
+    if kind != "llama3":
+        raise ValueError(f"rope_scaling type {kind!r}: only 'llama3' is provided")
+    factor, lo_f, hi_f = f32(scaling["factor"]), f32(scaling["low_freq_factor"]), f32(scaling["high_freq_factor"])
+    old = f32(scaling["original_max_position_embeddings"])
+    lo_wave, hi_wave = old / lo_f, old / hi_f
+    wave = f32(2 * np.pi) / inv
+    scaled = np.where(wave > lo_wave, inv / factor, inv)
+    smooth = (old / wave - lo_f) / (hi_f - lo_f)
+    smoothed = (f32(1) - smooth) * scaled / factor + smooth * scaled
+    medium = ~(wave < hi_wave) & ~(wave > lo_wave)
+    return np.where(medium, smoothed, scaled).astype(f32)
+
+
 # ---------------------------------------------------------------- Llama decode (C3 / C5)
+LLAMA31_ROPE_SCALING = {"type": "llama3", "factor": 8.0, "low_freq_factor": 1.0, "high_freq_factor": 4.0,
+                        "original_max_position_embeddings": 8192}
+
+
 @dataclass
 class LlamaConfig:
     layers: int = 32
@@ -79,16 +116,33 @@ class LlamaConfig:
     kv_heads: int | None = None  # grouped-query attention: KV heads shared by heads // kv_heads query heads each; None = heads
     kv_fp8: bool = False  # KV caches as FP8 E4M3 codes + per-layer f32 [KV heads] k / v scales (one token per step)
     int4_block: int = 0  # 32 / 64 / 128: the seven projections of every layer + the logits head as MatMulNBits (4-bit, symmetric)
+    rope_theta: float = 10000.0  # RoPE base
+    rope_scaling: dict | None = None  # None, or {"type": "llama3", factor, low_freq_factor, high_freq_factor,
+                                      # original_max_position_embeddings} (see rope_inv_freq)
 
     @property
     def n_kv(self) -> int:
         return self.heads if self.kv_heads is None else self.kv_heads
 
+    @property
+    def rope_default(self) -> bool:
+        """base 10000 without scaling: the RoPE nodes take no inv_freq table"""
+        return self.rope_theta == 10000.0 and self.rope_scaling is None
+
     @staticmethod
     def llama3_8b(batch=16, s_max=1024, dtype=BF16, layers=32, kv_fp8=False, int4_block=0):
-        """Llama-3-8B shape: 32 query heads over 8 KV heads (G = 4)."""
+        """Llama-3-8B shape: 32 query heads over 8 KV heads (G = 4).  A shape only: its RoPE is base 10000, not Llama-3's
+        500 000; `llama31_8b` has Llama-3.1's frequencies."""
         return LlamaConfig(layers=layers, d_model=4096, heads=32, kv_heads=8, head_dim=128, ffn=14336, vocab=128256,
                            s_max=s_max, batch=batch, dtype=dtype, kv_fp8=kv_fp8, int4_block=int4_block)
+
+    @staticmethod
+    def llama31_8b(batch=16, s_max=1024, dtype=BF16, layers=32, kv_fp8=False, int4_block=0):
+        """Llama-3.1-8B: the Llama-3-8B shape with its RoPE, base 500 000 and llama3 scaling (factor 8, low / high frequency
+        factors 1 / 4, original context 8192)."""
+        return LlamaConfig(layers=layers, d_model=4096, heads=32, kv_heads=8, head_dim=128, ffn=14336, vocab=128256,
+                           s_max=s_max, batch=batch, dtype=dtype, kv_fp8=kv_fp8, int4_block=int4_block,
+                           rope_theta=500000.0, rope_scaling=dict(LLAMA31_ROPE_SCALING))
 
     @staticmethod
     def tiny(dtype=BF16, layers=2, batch=4, kv_fp8=False):
@@ -160,6 +214,8 @@ def build_llama_decode(h, cfg: LlamaConfig, world: int = 1, rank: int = 0, seq: 
     dl, dkv = H * dh, Hkv * dh  # local attention widths of q and of k / v
     _require_head_width(h, dh)
     rope_kw = {} if dh == 128 else {"dim_head": dh}  # 128-wide graphs make the reference's RoPE call
+    if not cfg.rope_default:
+        _require_rope_table(h, cfg)
     g = LlamaGraph(cfg)
 
     def weight(name, shape, kind, shard=None):
@@ -197,6 +253,11 @@ def build_llama_decode(h, cfg: LlamaConfig, world: int = 1, rank: int = 0, seq: 
     g.input_ids.set_input()
     g.position_ids.set_input()
     emb = weight("embed", (V, d), "embed")
+    if not cfg.rope_default:  # one table, shared by every RoPE (replicated on every rank)
+        inv = h.tensor([dh // 2], F32)
+        inv.set_weight()
+        g.weights["rope.inv_freq"] = (inv, (dh // 2,), "inv_freq", None)
+        rope_kw["inv_freq"] = inv
     x = h.gather(emb, g.input_ids, None, 0)  # [B,seq,d]
     for li in range(cfg.layers):
         p = f"l{li}."
@@ -318,6 +379,9 @@ def fill_llama_weights_host(g: LlamaGraph, world: int = 1, rank: int = 0, seed: 
     for name, (t, shape, kind, shard) in g.weights.items():
         if kind == "scale":
             continue  # written together with its codes
+        if kind == "inv_freq":
+            t.copyin_numpy(rope_inv_freq(g.cfg.head_dim, g.cfg.rope_theta, g.cfg.rope_scaling))
+            continue
         if kind == "kv_scale":  # the scale the cache helpers quantise with (llama_kv_fp8_values)
             li, which = int(name[1:name.index(".")]), name[name.index(".") + 1]
             t.copyin_numpy(llama_kv_fp8_values(g.cfg, li, which, world, rank)[1])

@@ -560,13 +560,16 @@ class OnnxStub:
                                            a.get("stash_type", 1))
         elif op == "RMSNorm":
             T[out0] = h.RMSNorm(I(0), I(1), None)
-        elif op == "RoPE":  # optional int attribute dim_head (extension; absent = the reference's 128)
+        elif op == "RoPE":  # optional int attribute dim_head and optional input 2, inv_freq (extensions; absent = the reference's)
+            kw = {"inv_freq": I(2)} if len(nd.inputs) > 2 and nd.inputs[2] else {}
+            if kw and not getattr(h, "rope_inv_freq", False):
+                raise NotImplementedError(f"RoPE {nd.name}: {type(h).__name__} does not execute an inv_freq table")
             if "dim_head" in a and int(a["dim_head"]) != 128:
                 if int(a["dim_head"]) not in getattr(h, "head_widths", (128,)):
                     raise NotImplementedError(f"RoPE {nd.name}: {type(h).__name__} does not execute dim_head {a['dim_head']}")
-                T[out0] = h.RoPE(I(0), I(1), None, int(a["dim_head"]))
+                T[out0] = h.RoPE(I(0), I(1), None, int(a["dim_head"]), **kw)
             else:
-                T[out0] = h.RoPE(I(0), I(1), None)
+                T[out0] = h.RoPE(I(0), I(1), None, **kw)
         elif op == "AttentionKVCache":  # optional inputs 6, 7 (extension): k_scale / v_scale of FP8 E4M3 caches
             scales = {"k_scale": I(6), "v_scale": I(7)} if len(nd.inputs) > 6 else {}
             T[out0] = h.attentionKVCache(I(0), I(1), I(2), I(3), I(4), I(5), None, **scales)
@@ -774,10 +777,12 @@ class OnnxExporter:
                           {"epsilon": float(eps), "axis": int(axis), "stash_type": int(stash_type)})
 
     def RMSNorm(self, x, w, y): return self._emit("RMSNorm", [x, w], self.inner.RMSNorm(x.inner, w.inner, self._in(y)))
-    def RoPE(self, pos, x, y, dim_head=128):  # the attribute only when it is not the reference's 128: older files stay as they were
+    def RoPE(self, pos, x, y, dim_head=128, inv_freq=None):
+        # the attribute only when it is not the reference's 128, the third input only when given: older files stay as they were
         extra = [] if dim_head == 128 else [int(dim_head)]
-        return self._emit("RoPE", [pos, x], self.inner.RoPE(pos.inner, x.inner, self._in(y), *extra),
-                          {"dim_head": extra[0]} if extra else None)
+        kw = {} if inv_freq is None else {"inv_freq": inv_freq.inner}
+        return self._emit("RoPE", [pos, x] + ([inv_freq] if inv_freq is not None else []),
+                          self.inner.RoPE(pos.inner, x.inner, self._in(y), *extra, **kw), {"dim_head": extra[0]} if extra else None)
 
     def attentionKVCache(self, kc, vc, q, k, v, pos, y, k_scale=None, v_scale=None):
         # the FP8 caches' scales only when given: every 16-bit export stays as it was
@@ -931,7 +936,7 @@ def parallel_model(model, world: int, rank: int, new_handler=None) -> Model:
       * fed by an activation sharded on its last axis it is row-split, and a `ReduceSum(communicator=0)` node -- which the
         frontend lowers to AllReduceSum (onnx.py:917-923) -- makes the result replicated again; a Gemm bias is added once, after;
       * the last MatMul (the one producing a graph output) stays replicated, like embeddings, norms and the residual stream;
-      * placements flow through unary / binary ops, RoPE, Transpose (through the permutation), Split, AttentionKVCache (heads;
+      * placements flow through unary / binary ops, RoPE (its inv_freq table replicated), Transpose (through the permutation), Split, AttentionKVCache (heads;
         the cache INPUTS shrink on the head axis) and Reshape (the output axis whose row-major prefix product equals the
         sharded input axis' takes the division).
     The model is simplified first, so Reshape targets are plain initializers."""
