@@ -388,6 +388,26 @@ int it_b200_attention_kvcache_prompt(int dtype, void *k_cache, void *v_cache, co
                                      const void *position_id, int pos_flags, void *out, int B, int Hq, int Hkv, int S, int S_max,
                                      int D, void *stream);
 
+/* ---- Sliding-window attention (Mistral-7B-v0.1 and models trained like it).  window >= 1: the query at position P reads only
+ *      cache rows j with P - window < j <= P, its own row included (transformers' `kv_idx > q_idx - sliding_window`; the
+ *      original Mistral code keeps one row more: pass window + 1 for that).  Positions, clamping and the append are unchanged;
+ *      the cache is still indexed by absolute position, so S_max must cover the longest position.  Rows below a query's window
+ *      never reach its output, even when they hold NaN.  window 0 is no window: the same kernels as the unwindowed calls.
+ *      window < 0 is refused, before any launch.
+ *   _window: every decode variant in one call.  k_scale / v_scale NULL: 16-bit or fp32 caches, non-NULL: FP8 E4M3 caches
+ *      (it_b200_attention_kvcache_fp8); rope_pos NULL: no RoPE; inv_freq NULL: base 10000, else the table
+ *      (it_b200_attention_kvcache_gqa_freq, freq_dtype / freq_len checked alike).  A windowed head streams only the rows
+ *      [max(0, P - window + 1), P): min(P + 1, window) rows per step instead of P + 1.
+ *   _prompt_window: it_b200_attention_kvcache_prompt, query i of batch row b reading rows (p_b + i - window, p_b + i]. ---- */
+int it_b200_attention_kvcache_window(int dtype, void *k_cache, void *v_cache, const void *k_scale, const void *v_scale,
+                                     const void *q, const void *k, const void *v, const void *rope_pos, int rope_pos_dtype,
+                                     const void *inv_freq, int freq_dtype, int64_t freq_len, int window, const void *position_id,
+                                     int pos_flags, void *out, int B, int Hq, int Hkv, int S_max, int D, void *workspace,
+                                     int64_t workspace_bytes, void *stream);
+int it_b200_attention_kvcache_prompt_window(int dtype, void *k_cache, void *v_cache, const void *q, const void *k, const void *v,
+                                            const void *position_id, int pos_flags, void *out, int B, int Hq, int Hkv, int S,
+                                            int S_max, int D, int window, void *stream);
+
 /* ---- Fused prefill attention (q-len > 1) on wgmma (SURVEY 8(f-3); attention_prefill.cu):
  *      out[b,h] = softmax((q . k^T) (/ or *) scale + mask) . v, q / k / v / out [B, H, S, D] f16 / bf16, D = 64 or 128.
  *      Replaces the chain the frontend lowers multi-token attention to -- Transpose(k) -> MatMul (matmul.cc:66-211) ->

@@ -97,6 +97,9 @@ _SIGS = {
     "it_b200_attention_kvcache_fp8_freq": (c_int, [c_int, vp, vp, vp, vp, vp, vp, vp, vp, c_int, vp, c_int, vp, c_int, c_int64, vp,
                                                    c_int, c_int, c_int, c_int, c_int, vp, c_int64, vp]),
     "it_b200_attention_kvcache_prompt": (c_int, [c_int, vp, vp, vp, vp, vp, vp, c_int, vp] + [c_int] * 6 + [vp]),
+    "it_b200_attention_kvcache_window": (c_int, [c_int, vp, vp, vp, vp, vp, vp, vp, vp, c_int, vp, c_int, c_int64, c_int, vp, c_int,
+                                                 vp, c_int, c_int, c_int, c_int, c_int, vp, c_int64, vp]),
+    "it_b200_attention_kvcache_prompt_window": (c_int, [c_int, vp, vp, vp, vp, vp, vp, c_int, vp] + [c_int] * 7 + [vp]),
     "it_b200_attention_prefill": (c_int, [c_int, vp, vp, vp, vp, c_int, c_int, c_int, c_int, c_int, vp, c_int, vp, c_int64, c_int64,
                                           c_int64, c_int64, vp]),
     "it_b200_attention_prefill_strided": (c_int, [c_int, vp, vp, vp, vp] + [c_int] * 5 + [vp, vp, vp, vp, vp, c_int, vp, c_int64, c_int64, c_int64, c_int64, vp]),

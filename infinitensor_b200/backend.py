@@ -309,6 +309,7 @@ class GraphHandler:
 
     head_widths = (64, 128)  # decode attention / RoPE head widths (64: extension; the reference's are 128)
     rope_inv_freq = True  # RoPE takes the model's frequencies as an optional inv_freq input (extension)
+    sliding_window = True  # AttentionKVCache takes a sliding window (extension)
 
     def __init__(self, runtime: CudaRuntime):
         if not isinstance(runtime, CudaRuntime):
@@ -433,17 +434,20 @@ class GraphHandler:
         return self._op1("Concat", list(inputs), output, [dim])
 
     def attentionKVCache(self, input_k_cache, input_v_cache, input_q, input_k, input_v, position_id, output_matmul,
-                         per_row_positions=False, k_scale=None, v_scale=None):
+                         per_row_positions=False, k_scale=None, v_scale=None, window=0):
         """per_row_positions (extension, SURVEY 8(f-3)): batch row b attends up to / appends at position_id[b]; the default is
         the reference's rule -- element 0 for every row (attention_kvcache.cu:17).
         k_scale / v_scale (extension): the caches hold FP8 E4M3 codes (dtype 17), element value e4m3(code) * scale[KV head];
-        both f32 [Hkv], given together, exactly when the caches are FP8.  One token per step, f16 / bf16 q / k / v."""
+        both f32 [Hkv], given together, exactly when the caches are FP8.  One token per step, f16 / bf16 q / k / v.
+        window (extension): sliding-window attention, the query at position P attends over cache rows (P - window, P] only
+        (HF's sliding_window); 0 = no window.  Decode and prompt steps, every cache type; a negative window is refused."""
         ins = [input_k_cache, input_v_cache, input_q, input_k, input_v, position_id]
         if (k_scale is None) != (v_scale is None):
             raise ValueError("attentionKVCache: k_scale and v_scale go together")
         if k_scale is not None:
             ins += [k_scale, v_scale]
-        return self._op1("AttentionKVCache", ins, output_matmul, [1] if per_row_positions else [])
+        attrs = [int(bool(per_row_positions)), int(window)] if window else ([1] if per_row_positions else [])
+        return self._op1("AttentionKVCache", ins, output_matmul, attrs)
 
     def RoPE(self, pos, input, output, dim_head=128, inv_freq=None):
         """dim_head (extension): rotate-half within heads of this width; the reference fixes it at 128 (rope.cc:25).

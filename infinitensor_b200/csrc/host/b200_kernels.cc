@@ -575,6 +575,14 @@ void runAttentionRope(const Operator &ropeQ, const Operator &ropeK, const Operat
     int64_t wsb = it_b200_attention_kvcache_workspace(d[0], hq, d[2], d[3]);
     void *ws = wsb ? RT(ctx)->getWorkspace((size_t)wsb) : nullptr;
     const int flags = attnPosFlags(att, rpos, freq);
+    if (const int window = as<AttentionKVCacheObj>(att)->getWindow()) {  // sliding window: every cache type and RoPE mode
+        const bool fp8 = as<AttentionKVCacheObj>(att)->isFp8Cache();
+        CK(it_b200_attention_kvcache_window(DTI(qpre), P(kc), P(vc), fp8 ? P(att->getInputs(6)) : nullptr, fp8 ? P(att->getInputs(7)) : nullptr,
+                                            P(qpre), P(kpre), P(v), P(rpos), DTI(rpos), freq ? P(freq) : nullptr, freq ? DTI(freq) : 0,
+                                            freq ? (int64_t)freq->size() : 0, window, P(pos), flags, P(att->getOutput()), d[0], hq, d[1],
+                                            d[2], d[3], ws, wsb, S()), att);
+        return;
+    }
     if (freq) {  // the model's own frequencies
         const int64_t nf = (int64_t)freq->size();
         if (as<AttentionKVCacheObj>(att)->isFp8Cache())
@@ -841,6 +849,23 @@ class AttentionKVCacheB200 : public CudaKernelWithoutConfig {
              v = op->getInputs(4), pos = op->getInputs(5);
         const auto &d = kc->getDims();
         const int hq = q->getDims()[1];  // = G x the caches' d[1] KV heads
+#ifndef ITB_SEAM_A
+        if (const int window = as<AttentionKVCacheObj>(op)->getWindow()) {  // sliding window (the reference's operator has none)
+            const int seq = q->getDims()[2];
+            if (seq > 1) {
+                CK(it_b200_attention_kvcache_prompt_window(DTI(q), P(kc), P(vc), P(q), P(k), P(v), P(pos), b200::attnPosFlags(op, nullptr),
+                                                           P(op->getOutput()), d[0], hq, d[1], seq, d[2], d[3], window, S()), op);
+                return;
+            }
+            int64_t wsb = it_b200_attention_kvcache_workspace(d[0], hq, d[2], d[3]);
+            void *ws = wsb ? RT(ctx)->getWorkspace((size_t)wsb) : nullptr;
+            const bool fp8 = kc->getDType() == DataType::Float8E4M3FN;
+            CK(it_b200_attention_kvcache_window(DTI(q), P(kc), P(vc), fp8 ? P(op->getInputs(6)) : nullptr, fp8 ? P(op->getInputs(7)) : nullptr,
+                                                P(q), P(k), P(v), nullptr, 0, nullptr, 0, 0, window, P(pos), b200::attnPosFlags(op, nullptr),
+                                                P(op->getOutput()), d[0], hq, d[1], d[2], d[3], ws, wsb, S()), op);
+            return;
+        }
+#endif
         if (const int seq = q->getDims()[2]; seq > 1) {  // a prompt chunk: append + causal attention over the cache
             CK(it_b200_attention_kvcache_prompt(DTI(q), P(kc), P(vc), P(q), P(k), P(v), P(pos),
 #ifdef ITB_SEAM_A

@@ -136,15 +136,16 @@ static TensorVec attentionInputs(TensorVec v, Tensor kScale, Tensor vScale) {
 }
 AttentionKVCacheObj::AttentionKVCacheObj(GraphObj *graph, Tensor input_k_cache, Tensor input_v_cache,
                                          Tensor input_q, Tensor input_k, Tensor input_v, Tensor position_id,
-                                         Tensor output_matmul, bool perRowPositions, Tensor k_scale, Tensor v_scale)
+                                         Tensor output_matmul, bool perRowPositions, Tensor k_scale, Tensor v_scale, int window)
     : OperatorObj(OpType::AttentionKVCache,
                   attentionInputs({input_k_cache, input_v_cache, input_q, input_k, input_v, position_id}, k_scale, v_scale),
                   {output_matmul}),
-      perRowPositions(perRowPositions) {
+      perRowPositions(perRowPositions), window(window) {
     IT_ASSERT(checkValid(graph));
 }
 std::optional<vector<Shape>> AttentionKVCacheObj::inferShape(const TensorVec &ins) {
     IT_ASSERT(ins.size() == 6 || ins.size() == 8, "AttentionKVCache takes 6 inputs, or 8 with an FP8 cache's scales");
+    IT_ASSERT(window >= 0, "AttentionKVCache: window " + std::to_string(window) + " is negative (0 = no window)");
     const bool fp8k = ins[0]->getDType() == DataType::Float8E4M3FN, fp8v = ins[1]->getDType() == DataType::Float8E4M3FN;
     // FP8 E4M3 caches (extension): k_scale / v_scale f32 [Hkv] are inputs 6 and 7, present exactly when the caches are FP8
     IT_ASSERT(fp8k == fp8v, "AttentionKVCache: k_cache and v_cache must both be FP8 or neither");

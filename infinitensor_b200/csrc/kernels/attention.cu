@@ -128,14 +128,14 @@ template <typename KT> __device__ __forceinline__ auto ld_cache_row(const KT *p)
 
 constexpr int AS_MAX_B = 1024;  // batch rows whose (position, chunk count) the CTA keeps in shared memory
 
-template <typename T, typename KT, int D, int WARPS, int U, int ROPE>
+template <typename T, typename KT, int D, int WARPS, int U, int ROPE, bool WIN = false>
 __device__ __forceinline__ void
     attn_stream_body(KT *__restrict__ kcache, KT *__restrict__ vcache, const T *__restrict__ q,
                        const T *__restrict__ kin, const T *__restrict__ vin, const void *__restrict__ position_id,
                        int pos_flags, T *__restrict__ out, int Smax, int BH, float *__restrict__ partial,
                        int slots_per_head, int *__restrict__ tickets, const void *__restrict__ rope_pos,
                        int rope_pos_dtype, int H, const float *__restrict__ k_scale, const float *__restrict__ v_scale,
-                       const float *__restrict__ inv_freq) {
+                       const float *__restrict__ inv_freq, int window = 0) {
     using C = RowCfg<KT, D>;
     constexpr int EPL = C::EPL, LPR = C::LPR, RPW = C::RPW;
     constexpr int VE = Vec16<T>::N, NV = EPL / VE;            // a lane's EPL activations: NV 16-byte vectors (FP8: 2)
@@ -160,6 +160,10 @@ __device__ __forceinline__ void
     // the producer starts streaming while the previous kernel of the chain drains.
     if (pos_flags & ITB_POS_IN_STEP) pdl_wait();
     const int Bn = BH / H;
+    // span(p): the cache rows read below position p -- all p of them, or (WIN) the last window - 1, from lo = p - span(p).
+    // Units, offsets and the dealing count from lo, so a windowed head at p runs exactly as an unwindowed one at span(p)
+    // over the cache rows from lo up
+    auto span = [&](int p) { return WIN ? min(p, window - 1) : p; };
     if (threadIdx.x == 0) {
         for (int s = 0; s < AS_STAGES; ++s) {
             mbar_init(&full[s], 1);
@@ -177,7 +181,7 @@ __device__ __forceinline__ void
         int acc = 0;
         for (int b = 0; b < Bn; ++b) {
             s_pre[b] = acc;
-            acc += H * (s_pos[b] / CH + 1);  // chunks per head of row b; the last one holds rows [.., pos) + the appended row
+            acc += H * (span(s_pos[b]) / CH + 1);  // chunks per head of row b; the last one holds rows [.., pos) + the appended row
         }
         s_pre[Bn] = acc;
     }
@@ -198,7 +202,7 @@ __device__ __forceinline__ void
         brow = 0;
         while (brow + 1 < Bn && s_pre[brow + 1] <= u0) ++brow;
         pos = s_pos[brow];
-        nch = pos / CH + 1;
+        nch = span(pos) / CH + 1;
         const int r = (int)(u0 - s_pre[brow]);
         bh = brow * H + r / nch;
         c = r % nch;
@@ -210,7 +214,7 @@ __device__ __forceinline__ void
             if (bh % H == 0 && bh < BH) {
                 brow = bh / H;
                 pos = s_pos[brow];
-                nch = pos / CH + 1;
+                nch = span(pos) / CH + 1;
             }
         }
     };
@@ -222,10 +226,10 @@ __device__ __forceinline__ void
             int st = 0, ph = 0;
             for (int it = 0; it < nunits; ++it) {
                 mbar_wait(&empty[st], ph ^ 1);
-                const int rows = min(CH, pos - c * CH);
+                const int rows = min(CH, span(pos) - c * CH);
                 if (rows > 0) {
                     const uint32_t bytes = (uint32_t)rows * D * (uint32_t)sizeof(KT);
-                    const int64_t off = ((int64_t)bh * Smax + (int64_t)c * CH) * D;
+                    const int64_t off = ((int64_t)bh * Smax + (pos - span(pos)) + (int64_t)c * CH) * D;
                     mbar_expect_tx(&full[st], 2 * bytes);
                     bulk_load_1d(ring + (size_t)st * 2 * CHUNK_BYTES, kcache + off, bytes, &full[st], policy);
                     bulk_load_1d(ring + (size_t)st * 2 * CHUNK_BYTES + CHUNK_BYTES, vcache + off, bytes, &full[st], policy);
@@ -286,7 +290,7 @@ __device__ __forceinline__ void
 #pragma unroll
                 for (int h = 0; h < NV; ++h) qf[VE * h + j] = to_f(qv[h].v[j]) * qs;
         }
-        const int nvalid = pos - c * CH;  // cache rows of this chunk that exist (<= 0: only the appended row)
+        const int nvalid = span(pos) - c * CH;  // cache rows of this chunk that exist (<= 0: only the appended row)
         const unsigned char *kb = ring + (size_t)st * 2 * CHUNK_BYTES, *vb = kb + CHUNK_BYTES;
         mbar_wait(&full[st], ph);
 #ifndef ATTN_DBG_NOCOMPUTE  // (debug builds only: measures the bare HBM -> smem ring)
@@ -534,13 +538,13 @@ template <typename T, int D, typename KT = T> struct GqaCfg {  // KT: the cache 
     static constexpr int PLD = CH + 16 / (int)sizeof(T);
 };
 
-template <typename T, typename KT, int D, int QT, int ROPE, typename... Scale>
+template <typename T, typename KT, int D, int QT, int ROPE, bool WIN = false, typename... Scale>
 __device__ __forceinline__ void
     attn_gqa_body(KT *__restrict__ kcache, KT *__restrict__ vcache, const T *__restrict__ q,
                     const T *__restrict__ kin, const T *__restrict__ vin, const void *__restrict__ position_id,
                     int pos_flags, T *__restrict__ out, int Smax, int Bn, int Hkv, int G, int NQG,
                     float *__restrict__ partial, int slots_per_head, int *__restrict__ tickets, const void *__restrict__ rope_pos, int rope_pos_dtype,
-                    const float *__restrict__ inv_freq, const Scale *__restrict__... kv_scale) {
+                    const float *__restrict__ inv_freq, int window, const Scale *__restrict__... kv_scale) {
     // kv_scale: k_scale, v_scale for an FP8 cache, nothing for the others (unused scale parameters alone change how the
     // unquantised kernels compile)
     using C = RowCfg<T, D>;  // row-load layout of q and the appended k / v
@@ -571,6 +575,7 @@ __device__ __forceinline__ void
                                            : read_pos<int32_t>(position_id, per_row ? b : 0);
         return min(max(p, 0), Smax - 1);
     };
+    auto span = [&](int p) { return WIN ? min(p, window - 1) : p; };  // (see attn_stream_body)
     if (threadIdx.x == 0) {
         for (int s = 0; s < AS_STAGES; ++s) {
             mbar_init(&full[s], 1);
@@ -584,7 +589,7 @@ __device__ __forceinline__ void
         reinterpret_cast<uint4 *>(ring)[i] = make_uint4(0, 0, 0, 0);
     fence_proxy_async();
     const int HV = Hkv * NQG;  // (KV head, query group) segments per batch row
-    for (int b = threadIdx.x; b < Bn; b += blockDim.x) s_pre[b] = HV * (pos_of(b) / CH + 1);
+    for (int b = threadIdx.x; b < Bn; b += blockDim.x) s_pre[b] = HV * (span(pos_of(b)) / CH + 1);
     __syncthreads();
     if (threadIdx.x == 0) {
         int acc = 0;
@@ -608,7 +613,7 @@ __device__ __forceinline__ void
         brow = 0;
         while (brow + 1 < Bn && s_pre[brow + 1] <= u0) ++brow;
         pos = pos_of(brow);
-        nch = pos / CH + 1;
+        nch = span(pos) / CH + 1;
         const int r = (int)(u0 - s_pre[brow]);
         bh = brow * HV + r / nch;
         c = r % nch;
@@ -620,7 +625,7 @@ __device__ __forceinline__ void
             if (bh % HV == 0 && bh < BH) {
                 brow = bh / HV;
                 pos = pos_of(brow);
-                nch = pos / CH + 1;
+                nch = span(pos) / CH + 1;
             }
         }
     };
@@ -632,10 +637,10 @@ __device__ __forceinline__ void
             int st = 0, ph = 0;
             for (int it = 0; it < nunits; ++it) {
                 mbar_wait(&empty[st], ph ^ 1);
-                const int rows = min(CH, pos - c * CH);
+                const int rows = min(CH, span(pos) - c * CH);
                 if (rows > 0) {
                     const uint32_t bytes = (uint32_t)rows * D * (uint32_t)sizeof(KT);
-                    const int64_t off = ((int64_t)(bh / NQG) * Smax + (int64_t)c * CH) * D;
+                    const int64_t off = ((int64_t)(bh / NQG) * Smax + (pos - span(pos)) + (int64_t)c * CH) * D;
                     mbar_expect_tx(&full[st], 2 * bytes);
                     bulk_load_1d(ring + (size_t)st * 2 * CHUNK_BYTES, kcache + off, bytes, &full[st], policy);
                     bulk_load_1d(ring + (size_t)st * 2 * CHUNK_BYTES + CHUNK_BYTES, vcache + off, bytes, &full[st], policy);
@@ -702,7 +707,7 @@ __device__ __forceinline__ void
             }
             named_bar_sync(1, CONSUMERS);
         }
-        const int nvalid = pos - c * CH;  // cache rows of this chunk below the position (last chunk: < CH)
+        const int nvalid = span(pos) - c * CH;  // cache rows of this chunk below the position (last chunk: < CH)
         const bool last_chunk = c == nch - 1;
         KT *ks = reinterpret_cast<KT *>(ring + (size_t)st * 2 * CHUNK_BYTES), *vs = ks + CH * D;
         mbar_wait(&full[st], ph);
@@ -1104,11 +1109,11 @@ __global__ void __launch_bounds__((WARPS + 1) * 32, AS_CTAS_PER_SM) attn_stream6
 }
 template <typename T, int QT, bool ROPE>
 __global__ void __launch_bounds__((GQ_WARPS + 1) * 32, AS_CTAS_PER_SM) attn_gqa_kernel(ITB_ATTN_GQA_ARGS(T)) {
-    attn_gqa_body<T, T, 128, QT, ROPE ? ROPE_BASE : ROPE_NONE>(ITB_ATTN_GQA_PASS, nullptr);  // (pdl_trigger / pdl_wait inside)
+    attn_gqa_body<T, T, 128, QT, ROPE ? ROPE_BASE : ROPE_NONE>(ITB_ATTN_GQA_PASS, nullptr, 0);  // (pdl_trigger / pdl_wait inside)
 }
 template <typename T, int QT, bool ROPE>
 __global__ void __launch_bounds__((GQ_WARPS + 1) * 32, AS_CTAS_PER_SM) attn_gqa64_kernel(ITB_ATTN_GQA_ARGS(T)) {
-    attn_gqa_body<T, T, 64, QT, ROPE ? ROPE_BASE : ROPE_NONE>(ITB_ATTN_GQA_PASS, nullptr);  // (pdl_trigger / pdl_wait inside)
+    attn_gqa_body<T, T, 64, QT, ROPE ? ROPE_BASE : ROPE_NONE>(ITB_ATTN_GQA_PASS, nullptr, 0);  // (pdl_trigger / pdl_wait inside)
 }
 
 // FP8 E4M3 caches: uint8_t codes + one fp32 scale per KV head, f16 / bf16 activations, both widths in one name each
@@ -1120,7 +1125,7 @@ __global__ void __launch_bounds__((WARPS + 1) * 32, AS_CTAS_PER_SM)
 template <typename T, int D, int QT, bool ROPE>
 __global__ void __launch_bounds__((GQ_WARPS + 1) * 32, AS_CTAS_PER_SM)
     attn_gqa_kv8_kernel(ITB_ATTN_GQA_ARGS(uint8_t), const float *__restrict__ k_scale, const float *__restrict__ v_scale) {
-    attn_gqa_body<T, uint8_t, D, QT, ROPE ? ROPE_BASE : ROPE_NONE>(ITB_ATTN_GQA_PASS, nullptr, k_scale, v_scale);  // (pdl_trigger / pdl_wait inside)
+    attn_gqa_body<T, uint8_t, D, QT, ROPE ? ROPE_BASE : ROPE_NONE>(ITB_ATTN_GQA_PASS, nullptr, 0, k_scale, v_scale);  // (pdl_trigger / pdl_wait inside)
 }
 
 // RoPE from an inv_freq table: one name per body for every cache type and width (k_scale / v_scale: FP8 caches only)
@@ -1134,8 +1139,24 @@ template <typename T, typename KT, int D, int QT>
 __global__ void __launch_bounds__((GQ_WARPS + 1) * 32, AS_CTAS_PER_SM)
     attn_gqa_freq_kernel(ITB_ATTN_GQA_ARGS(KT), const float *__restrict__ inv_freq, const float *__restrict__ k_scale,
                          const float *__restrict__ v_scale) {
-    if constexpr (KV8<KT>) attn_gqa_body<T, KT, D, QT, ROPE_TABLE>(ITB_ATTN_GQA_PASS, inv_freq, k_scale, v_scale);
-    else attn_gqa_body<T, KT, D, QT, ROPE_TABLE>(ITB_ATTN_GQA_PASS, inv_freq);  // (pdl_trigger / pdl_wait inside)
+    if constexpr (KV8<KT>) attn_gqa_body<T, KT, D, QT, ROPE_TABLE>(ITB_ATTN_GQA_PASS, inv_freq, 0, k_scale, v_scale);
+    else attn_gqa_body<T, KT, D, QT, ROPE_TABLE>(ITB_ATTN_GQA_PASS, inv_freq, 0);  // (pdl_trigger / pdl_wait inside)
+}
+
+// Sliding window (window >= 1): a query at position p reads cache rows (p - window, p], its own row included.  One name per
+// body for every cache type, width and RoPE mode (inv_freq: ROPE_TABLE only; k_scale / v_scale: FP8 caches only)
+template <typename T, typename KT, int D, int WARPS, int U, int ROPE>
+__global__ void __launch_bounds__((WARPS + 1) * 32, AS_CTAS_PER_SM)
+    attn_stream_win_kernel(ITB_ATTN_STREAM_ARGS(KT), const float *__restrict__ inv_freq, const float *__restrict__ k_scale,
+                           const float *__restrict__ v_scale, int window) {
+    attn_stream_body<T, KT, D, WARPS, U, ROPE, true>(ITB_ATTN_STREAM_PASS, k_scale, v_scale, inv_freq, window);  // (pdl_trigger / pdl_wait inside)
+}
+template <typename T, typename KT, int D, int QT, int ROPE>
+__global__ void __launch_bounds__((GQ_WARPS + 1) * 32, AS_CTAS_PER_SM)
+    attn_gqa_win_kernel(ITB_ATTN_GQA_ARGS(KT), const float *__restrict__ inv_freq, const float *__restrict__ k_scale,
+                        const float *__restrict__ v_scale, int window) {
+    if constexpr (KV8<KT>) attn_gqa_body<T, KT, D, QT, ROPE, true>(ITB_ATTN_GQA_PASS, inv_freq, window, k_scale, v_scale);
+    else attn_gqa_body<T, KT, D, QT, ROPE, true>(ITB_ATTN_GQA_PASS, inv_freq, window);  // (pdl_trigger / pdl_wait inside)
 }
 
 }  // namespace itb
@@ -1151,7 +1172,7 @@ extern "C" int64_t it_b200_attention_kvcache_workspace(int B, int H, int S_max, 
 template <typename T, typename KT, int D, int ROPE>
 static int launch_attn_stream(KT *kc, KT *vc, const T *q, const T *k, const T *v, const void *position_id, int pos_flags,
                               const void *rope_pos, int rope_pos_dtype, const float *inv_freq, T *out, int BH, int H, int S_max,
-                              float *workspace, const float *k_scale, const float *v_scale, cudaStream_t st) {
+                              float *workspace, const float *k_scale, const float *v_scale, int window, cudaStream_t st) {
     constexpr int WARPS = 8, U = 4;  // consumer warps x rows per lane and chunk
     constexpr int CH = WARPS * RowCfg<KT, D>::RPW * U;
     constexpr int smem = AS_STAGES * 2 * CH * D * (int)sizeof(KT);
@@ -1164,6 +1185,7 @@ static int launch_attn_stream(KT *kc, KT *vc, const T *q, const T *k, const T *v
         return launch(what, kern, {dim3(grid), dim3((WARPS + 1) * 32), smem, st}, kc, vc, q, k, v, position_id, pos_flags, out,
                       S_max, BH, workspace, stream_slots_per_head(S_max), tickets, rope_pos, rope_pos_dtype, H, extra...);
     };
+    if (window > 0) return go(attn_stream_win_kernel<T, KT, D, WARPS, U, ROPE>, inv_freq, k_scale, v_scale, window);
     constexpr bool R = ROPE == ROPE_BASE;
     if constexpr (ROPE == ROPE_TABLE) return go(attn_stream_freq_kernel<T, KT, D, WARPS, U>, inv_freq, k_scale, v_scale);
     else if constexpr (std::is_same_v<KT, uint8_t>) return go(attn_stream_kv8_kernel<T, D, WARPS, U, R>, k_scale, v_scale);
@@ -1173,7 +1195,7 @@ static int launch_attn_stream(KT *kc, KT *vc, const T *q, const T *k, const T *v
 template <typename T, typename KT, int D, int QT, int ROPE>
 static int launch_attn_gqa(KT *kc, KT *vc, const T *q, const T *k, const T *v, const void *position_id, int pos_flags,
                            const void *rope_pos, int rope_pos_dtype, const float *inv_freq, T *out, int B, int Hkv, int G, int S_max,
-                           float *workspace, const float *k_scale, const float *v_scale, cudaStream_t st) {
+                           float *workspace, const float *k_scale, const float *v_scale, int window, cudaStream_t st) {
     constexpr int CH = GqaCfg<T, D, KT>::CH;
     constexpr int smem = AS_STAGES * 2 * CH * D * (int)sizeof(KT);
     constexpr const char *what = KV8<KT> ? "AttentionKVCache(FP8 cache): grouped-query kernel" : "AttentionKVCache: grouped-query kernel";
@@ -1187,6 +1209,7 @@ static int launch_attn_gqa(KT *kc, KT *vc, const T *q, const T *k, const T *v, c
                       out, S_max, B, Hkv, G, nqg, workspace, stream_slots_per_head(S_max), tickets, rope_pos, rope_pos_dtype,
                       extra...);
     };
+    if (window > 0) return go(attn_gqa_win_kernel<T, KT, D, QT, ROPE>, inv_freq, k_scale, v_scale, window);
     constexpr bool R = ROPE == ROPE_BASE;
     if constexpr (ROPE == ROPE_TABLE) return go(attn_gqa_freq_kernel<T, KT, D, QT>, inv_freq, k_scale, v_scale);
     else if constexpr (std::is_same_v<KT, uint8_t>) return go(attn_gqa_kv8_kernel<T, D, QT, R>, k_scale, v_scale);
@@ -1199,7 +1222,8 @@ static int launch_attn_gqa(KT *kc, KT *vc, const T *q, const T *k, const T *v, c
 template <typename T, typename KT, int D>
 static int launch_attn_width(KT *kc, KT *vc, const T *q, const T *k, const T *v, const void *position_id, int pos_flags,
                              const void *rope_pos, int rope_pos_dtype, const float *inv_freq, T *out, int B, int Hq, int Hkv,
-                             int S_max, float *workspace, const float *k_scale, const float *v_scale, cudaStream_t st) {
+                             int S_max, float *workspace, const float *k_scale, const float *v_scale, int window,
+                             cudaStream_t st) {
     const int G = Hq / Hkv;
     auto go = [&](auto rope) {
         constexpr int R = decltype(rope)::value;
@@ -1207,12 +1231,12 @@ static int launch_attn_width(KT *kc, KT *vc, const T *q, const T *k, const T *v,
         const int rpd = R ? rope_pos_dtype : 0;
         if (G == 1)
             return launch_attn_stream<T, KT, D, R>(kc, vc, q, k, v, position_id, pos_flags, rp, rpd, inv_freq, out, B * Hq, Hq,
-                                                   S_max, workspace, k_scale, v_scale, st);
+                                                   S_max, workspace, k_scale, v_scale, window, st);
         if (G <= 16)
             return launch_attn_gqa<T, KT, D, 1, R>(kc, vc, q, k, v, position_id, pos_flags, rp, rpd, inv_freq, out, B, Hkv, G,
-                                                   S_max, workspace, k_scale, v_scale, st);
+                                                   S_max, workspace, k_scale, v_scale, window, st);
         return launch_attn_gqa<T, KT, D, 2, R>(kc, vc, q, k, v, position_id, pos_flags, rp, rpd, inv_freq, out, B, Hkv, G, S_max,
-                                               workspace, k_scale, v_scale, st);
+                                               workspace, k_scale, v_scale, window, st);
     };
     if (!rope_pos) return go(std::integral_constant<int, ROPE_NONE>{});
     return inv_freq ? go(std::integral_constant<int, ROPE_TABLE>{}) : go(std::integral_constant<int, ROPE_BASE>{});
@@ -1225,7 +1249,7 @@ static int attention_impl(int dtype, void *k_cache, void *v_cache, const void *q
                           const void *position_id, int pos_flags, const void *rope_pos, int rope_pos_dtype, void *out,
                           int B, int Hq, int Hkv, int S_max, int D, void *workspace, int64_t workspace_bytes,
                           void *stream, const float *k_scale = nullptr, const float *v_scale = nullptr,
-                          const float *inv_freq = nullptr) {
+                          const float *inv_freq = nullptr, int window = 0) {
     const int H = Hq;
     const int pos_dtype = pos_flags & 0xff;
     // 128: the reference's only width (attention_kvcache.cu:154); 64: GPT-2 / TinyLlama heads (extension)
@@ -1254,14 +1278,14 @@ static int attention_impl(int dtype, void *k_cache, void *v_cache, const void *q
             using T = decltype(tag);
             auto go = D == 64 ? launch_attn_width<T, uint8_t, 64> : launch_attn_width<T, uint8_t, 128>;
             return go((uint8_t *)k_cache, (uint8_t *)v_cache, (const T *)q, (const T *)k, (const T *)v, position_id, pos_flags,
-                      rope_pos, rope_pos_dtype, inv_freq, (T *)out, B, Hq, Hkv, S_max, (float *)workspace, k_scale, v_scale, st);
+                      rope_pos, rope_pos_dtype, inv_freq, (T *)out, B, Hq, Hkv, S_max, (float *)workspace, k_scale, v_scale, window, st);
         };
         return dtype == ITB_F16 ? fp8(__half{}) : fp8(__nv_bfloat16{});
     }
     ITB_DISPATCH_FLOAT(dtype, "AttentionKVCache", {
         auto go = D == 64 ? launch_attn_width<T, T, 64> : launch_attn_width<T, T, 128>;
         return go((T *)k_cache, (T *)v_cache, (const T *)q, (const T *)k, (const T *)v, position_id, pos_flags, rope_pos,
-                  rope_pos_dtype, inv_freq, (T *)out, B, Hq, Hkv, S_max, (float *)workspace, nullptr, nullptr, st);
+                  rope_pos_dtype, inv_freq, (T *)out, B, Hq, Hkv, S_max, (float *)workspace, nullptr, nullptr, window, st);
     });
     return 0;
 }
@@ -1331,4 +1355,22 @@ extern "C" int it_b200_attention_kvcache_fp8_freq(int dtype, void *k_cache, void
     return attention_impl(dtype, k_cache, v_cache, q, k, v, position_id, pos_flags, rope_pos, rope_pos_dtype, out, B, Hq, Hkv,
                           S_max, D, workspace, workspace_bytes, stream, (const float *)k_scale, (const float *)v_scale,
                           (const float *)inv_freq);
+}
+
+// Sliding-window decode over every cache type: k_scale / v_scale non-null, FP8 E4M3 codes; rope_pos non-null, RoPE folded in
+// (inv_freq non-null: the table's angles, else base 10000).  window >= 1: the query at position p reads rows (p - window, p];
+// window 0 runs the unwindowed kernels, as it_b200_attention_kvcache_gqa / _fp8 / _gqa_freq / _fp8_freq do
+extern "C" int it_b200_attention_kvcache_window(int dtype, void *k_cache, void *v_cache, const void *k_scale, const void *v_scale,
+                                                const void *q, const void *k, const void *v, const void *rope_pos, int rope_pos_dtype,
+                                                const void *inv_freq, int freq_dtype, int64_t freq_len, int window,
+                                                const void *position_id, int pos_flags, void *out, int B, int Hq, int Hkv, int S_max,
+                                                int D, void *workspace, int64_t workspace_bytes, void *stream) {
+    ITB_CHECK(window >= 0, "AttentionKVCache: window %d is negative", window);
+    ITB_CHECK(!k_scale == !v_scale, "AttentionKVCache(FP8 cache): k_scale and v_scale go together");
+    if (inv_freq && check_inv_freq(k_scale ? "AttentionKVCache(FP8 cache)+RoPE" : "AttentionKVCache+RoPE", rope_pos, inv_freq,
+                                   freq_dtype, freq_len, D))
+        return 1;
+    return attention_impl(dtype, k_cache, v_cache, q, k, v, position_id, pos_flags, rope_pos, rope_pos_dtype, out, B, Hq, Hkv,
+                          S_max, D, workspace, workspace_bytes, stream, (const float *)k_scale, (const float *)v_scale,
+                          (const float *)inv_freq, window);
 }

@@ -435,11 +435,11 @@ __global__ void __launch_bounds__(256) kvcache_append_kernel(T *__restrict__ kc,
     reinterpret_cast<uint4 *>(vc)[dst] = reinterpret_cast<const uint4 *>(v)[src];
 }
 
-template <typename T, int D>
-__global__ void __launch_bounds__(PK_THREADS, 1) attention_kvcache_prompt_kernel(const __grid_constant__ CUtensorMap mapQ,
-                                                                                 const __grid_constant__ CUtensorMap mapK,
-                                                                                 const __grid_constant__ CUtensorMap mapV,
-                                                                                 const PkArgs a) {
+// WIN (window >= 1): query i attends over rows (p_b + i - window, p_b + i] only.  Key tiles wholly below the tile's first query's
+// window are never loaded; the leading edge is masked per element like the causal one
+template <typename T, int D, bool WIN>
+__device__ __forceinline__ void prompt_body(const CUtensorMap &mapQ, const CUtensorMap &mapK, const CUtensorMap &mapV,
+                                            const PkArgs &a, int window) {
     constexpr int DG = D / 64;                  // 64-column groups of the head dim
     constexpr int TILE_BYTES = PK_BQ * D * 2;   // a Q, K or V tile: DG boxes of [64 rows x 64 columns], 128B swizzle
     constexpr int P_BYTES = PK_BQ * PK_BK * 2;  // P hi or lo: [64 queries x 64 keys], K-major, 128B swizzle
@@ -471,21 +471,24 @@ __global__ void __launch_bounds__(PK_THREADS, 1) attention_kvcache_prompt_kernel
     const int p = prompt_start(a.pos, a.pos_flags, b, a.S, a.Smax);
     const int last = p + min(i0 + PK_BQ - 1, a.S - 1);  // the tile's last query attends over rows 0 .. last
     const int nkt = last / PK_BK + 1;
+    const int lo0 = WIN ? max(p + i0 - window + 1, 0) : 0;  // the first row of the tile's first query's window
+    const int t0 = lo0 / PK_BK;                              // the first key tile loaded; tile t uses stage (t - t0) & 1
     const uint64_t pol = l2_policy_evict_last();
     auto load_kv = [&](int t) {
-        uint8_t *ks = kv_sm + (t & 1) * 2 * TILE_BYTES, *vs = ks + TILE_BYTES;
-        mbar_expect_tx(&bar_kv[t & 1], 2 * TILE_BYTES);
+        const int sg = (t - t0) & 1;
+        uint8_t *ks = kv_sm + sg * 2 * TILE_BYTES, *vs = ks + TILE_BYTES;
+        mbar_expect_tx(&bar_kv[sg], 2 * TILE_BYTES);
 #pragma unroll
         for (int g = 0; g < DG; ++g) {
-            tma_load_3d(ks + g * (PK_BK * 128), &mapK, &bar_kv[t & 1], g * 64, t * PK_BK, kvh, pol);
-            tma_load_3d(vs + g * (PK_BK * 128), &mapV, &bar_kv[t & 1], g * 64, t * PK_BK, kvh, pol);
+            tma_load_3d(ks + g * (PK_BK * 128), &mapK, &bar_kv[sg], g * 64, t * PK_BK, kvh, pol);
+            tma_load_3d(vs + g * (PK_BK * 128), &mapV, &bar_kv[sg], g * 64, t * PK_BK, kvh, pol);
         }
     };
     if (threadIdx.x == 0) {
         mbar_expect_tx(&bar_q, TILE_BYTES);
 #pragma unroll
         for (int g = 0; g < DG; ++g) tma_load_3d(q_sm + g * (PK_BQ * 128), &mapQ, &bar_q, g * 64, i0, bh, pol);
-        load_kv(0);
+        load_kv(t0);
     }
 
     // accumulator fragment: d[4 j + 2 r + e] is row 16 warp + lane / 4 + 8 r, column 8 j + 2 (lane % 4) + e
@@ -501,10 +504,11 @@ __global__ void __launch_bounds__(PK_THREADS, 1) attention_kvcache_prompt_kernel
     float m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};
     mbar_wait(&bar_q, 0);
 
-    for (int t = 0; t < nkt; ++t) {
-        if (threadIdx.x == 0 && t + 1 < nkt) load_kv(t + 1);  // (stage (t + 1) & 1 was released by the barrier closing t - 1)
-        uint8_t *ks = kv_sm + (t & 1) * 2 * TILE_BYTES, *vs = ks + TILE_BYTES;
-        mbar_wait(&bar_kv[t & 1], (t >> 1) & 1);
+    for (int t = t0; t < nkt; ++t) {
+        if (threadIdx.x == 0 && t + 1 < nkt) load_kv(t + 1);  // (stage (t + 1 - t0) & 1 was released by the barrier closing t - 1)
+        const int sg = (t - t0) & 1;
+        uint8_t *ks = kv_sm + sg * 2 * TILE_BYTES, *vs = ks + TILE_BYTES;
+        mbar_wait(&bar_kv[sg], ((t - t0) >> 1) & 1);
         const int j0 = t * PK_BK;
         // V rows past p_b + S - 1 (the last tile only) are cache contents this step does not own, possibly non-finite: they
         // meet P = 0 in the product, so they are zeroed here
@@ -512,6 +516,14 @@ __global__ void __launch_bounds__(PK_THREADS, 1) attention_kvcache_prompt_kernel
             const int r0 = p + a.S - j0;
             for (int c = threadIdx.x; c < (PK_BK - r0) * DG * 8; c += PK_THREADS) {
                 const int r = r0 + c / (DG * 8), g = (c / 8) % DG, ch = c % 8;
+                *reinterpret_cast<uint4 *>(vs + g * (PK_BK * 128) + r * 128 + ch * 16) = make_uint4(0, 0, 0, 0);
+            }
+            fence_proxy_async();
+        }
+        // likewise V rows below the first query's window (the first tile only): no query of the tile attends to them
+        if (WIN && j0 < lo0) {
+            for (int c = threadIdx.x; c < (lo0 - j0) * DG * 8; c += PK_THREADS) {
+                const int r = c / (DG * 8), g = (c / 8) % DG, ch = c % 8;
                 *reinterpret_cast<uint4 *>(vs + g * (PK_BK * 128) + r * 128 + ch * 16) = make_uint4(0, 0, 0, 0);
             }
             fence_proxy_async();
@@ -531,6 +543,7 @@ __global__ void __launch_bounds__(PK_THREADS, 1) attention_kvcache_prompt_kernel
         wg_wait<0>();
 
         const bool diag = j0 + PK_BK - 1 > p + i0;  // some key of the tile lies past the first query's limit
+        const bool lead = WIN && j0 <= last - window;  // some key of the tile lies below the last query's window
 #pragma unroll
         for (int r = 0; r < 2; ++r) {
             float mx = m[r];
@@ -539,11 +552,15 @@ __global__ void __launch_bounds__(PK_THREADS, 1) attention_kvcache_prompt_kernel
 #pragma unroll
                 for (int e = 0; e < 2; ++e) {
                     float &x = s[4 * j + 2 * r + e];
-                    x = (diag && j0 + 8 * j + fc + e > lim[r]) ? -INFINITY : x * kScale;
+                    const int key = j0 + 8 * j + fc + e;
+                    x = ((diag && key > lim[r]) || (lead && key <= lim[r] - window)) ? -INFINITY : x * kScale;
                     mx = fmaxf(mx, x);
                 }
             mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
-            mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));  // finite: key 0 of tile 0 is in every row
+            mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));  // unwindowed, finite: key 0 of tile 0 is in every row
+            // windowed, a row may have met only masked keys so far (m = mx = -inf): its exponentials subtract 0 instead, so
+            // that its weights and the correction stay 0 rather than exp(-inf + inf) = NaN, and m stays -inf
+            const float mxe = WIN && mx == -INFINITY ? 0.f : mx;
             const int prow = fr + 8 * r;
             uint8_t *hrow = ph_sm + prow * 128, *lrow = pl_sm + prow * 128;
             float sum = 0.f;
@@ -552,7 +569,7 @@ __global__ void __launch_bounds__(PK_THREADS, 1) attention_kvcache_prompt_kernel
                 __align__(4) T hi[2], lo[2];
 #pragma unroll
                 for (int e = 0; e < 2; ++e) {
-                    const float pr = expf(s[4 * j + 2 * r + e] - mx);  // masked: exp(-inf) = 0
+                    const float pr = expf(s[4 * j + 2 * r + e] - mxe);  // masked: exp(-inf) = 0
                     hi[e] = from_f<T>(pr);
                     lo[e] = from_f<T>(pr - to_f(hi[e]));
                     sum += pr;
@@ -564,7 +581,7 @@ __global__ void __launch_bounds__(PK_THREADS, 1) attention_kvcache_prompt_kernel
             }
             sum += __shfl_xor_sync(0xffffffffu, sum, 1);
             sum += __shfl_xor_sync(0xffffffffu, sum, 2);
-            const float corr = expf(m[r] - mx);  // m = -inf (first tile): 0, and o, l are still 0
+            const float corr = expf(m[r] - mxe);  // m = -inf (first tile): 0, and o, l are still 0
             l[r] = l[r] * corr + sum;
             m[r] = mx;
 #pragma unroll
@@ -613,7 +630,22 @@ __global__ void __launch_bounds__(PK_THREADS, 1) attention_kvcache_prompt_kernel
 }
 
 template <typename T, int D>
-static int launch_prompt(void *kc, void *vc, const void *q, const void *k, const void *v, const PkArgs &a, int B,
+__global__ void __launch_bounds__(PK_THREADS, 1) attention_kvcache_prompt_kernel(const __grid_constant__ CUtensorMap mapQ,
+                                                                                 const __grid_constant__ CUtensorMap mapK,
+                                                                                 const __grid_constant__ CUtensorMap mapV,
+                                                                                 const PkArgs a) {
+    prompt_body<T, D, false>(mapQ, mapK, mapV, a, 0);  // (pdl_trigger / pdl_wait inside)
+}
+template <typename T, int D>
+__global__ void __launch_bounds__(PK_THREADS, 1) attention_kvcache_prompt_win_kernel(const __grid_constant__ CUtensorMap mapQ,
+                                                                                     const __grid_constant__ CUtensorMap mapK,
+                                                                                     const __grid_constant__ CUtensorMap mapV,
+                                                                                     const PkArgs a, int window) {
+    prompt_body<T, D, true>(mapQ, mapK, mapV, a, window);  // (pdl_trigger / pdl_wait inside)
+}
+
+template <typename T, int D>
+static int launch_prompt(void *kc, void *vc, const void *q, const void *k, const void *v, const PkArgs &a, int B, int window,
                          cudaStream_t st) {
     const int64_t chunks = (int64_t)a.S * D / 8;
     if (launch("AttentionKVCache prompt: append", kvcache_append_kernel<T>,
@@ -626,6 +658,9 @@ static int launch_prompt(void *kc, void *vc, const void *q, const void *k, const
         !make_tma_3d_b16(&mv, vc, (uint64_t)B * a.Hkv, (uint64_t)a.Smax, D, D, (uint64_t)a.Smax * D, PK_BK, 64))
         ITB_FAIL("AttentionKVCache prompt: cuTensorMapEncodeTiled failed");
     const int smem = 5 * PK_BQ * D * 2 + 2 * PK_BQ * PK_BK * 2 + 1024;
+    if (window > 0)
+        return launch("AttentionKVCache prompt (window)", attention_kvcache_prompt_win_kernel<T, D>,
+                      {dim3((a.S + PK_BQ - 1) / PK_BQ, B * a.Hq), dim3(PK_THREADS), smem, st}, mq, mk, mv, a, window);
     return launch("AttentionKVCache prompt", attention_kvcache_prompt_kernel<T, D>,
                   {dim3((a.S + PK_BQ - 1) / PK_BQ, B * a.Hq), dim3(PK_THREADS), smem, st}, mq, mk, mv, a);
 }
@@ -709,10 +744,10 @@ extern "C" int it_b200_attention_prefill_strided(int dtype, const void *q, const
     return D == 64 ? launch_ap<__half, 64>(q, k, v, a, st, &sq, &sk, &sv) : launch_ap<__half, 128>(q, k, v, a, st, &sq, &sk, &sv);
 }
 
-// AttentionKVCache over S >= 1 new tokens per batch row (S = 1 is one decode step, served by the same two launches)
-extern "C" int it_b200_attention_kvcache_prompt(int dtype, void *k_cache, void *v_cache, const void *q, const void *k,
-                                                const void *v, const void *position_id, int pos_flags, void *out, int B,
-                                                int Hq, int Hkv, int S, int S_max, int D, void *stream) {
+// AttentionKVCache over S >= 1 new tokens per batch row (S = 1 is one decode step, served by the same two launches); window >= 1
+// limits query i to rows (p_b + i - window, p_b + i]
+static int prompt_impl(int dtype, void *k_cache, void *v_cache, const void *q, const void *k, const void *v, const void *position_id,
+                       int pos_flags, void *out, int B, int Hq, int Hkv, int S, int S_max, int D, int window, void *stream) {
     ITB_CHECK(dtype == ITB_F16 || dtype == ITB_BF16, "AttentionKVCache prompt: dtype %d must be f16 / bf16 (no fp32 prefill)", dtype);
     ITB_CHECK(D == 64 || D == 128, "AttentionKVCache prompt: head dim %d must be 64 or 128", D);
     const int pos_dtype = pos_flags & 0xff;
@@ -735,8 +770,21 @@ extern "C" int it_b200_attention_kvcache_prompt(int dtype, void *k_cache, void *
     a.Smax = S_max;
     auto st = (cudaStream_t)stream;
     if (dtype == ITB_BF16)
-        return D == 64 ? launch_prompt<__nv_bfloat16, 64>(k_cache, v_cache, q, k, v, a, B, st)
-                       : launch_prompt<__nv_bfloat16, 128>(k_cache, v_cache, q, k, v, a, B, st);
-    return D == 64 ? launch_prompt<__half, 64>(k_cache, v_cache, q, k, v, a, B, st)
-                   : launch_prompt<__half, 128>(k_cache, v_cache, q, k, v, a, B, st);
+        return D == 64 ? launch_prompt<__nv_bfloat16, 64>(k_cache, v_cache, q, k, v, a, B, window, st)
+                       : launch_prompt<__nv_bfloat16, 128>(k_cache, v_cache, q, k, v, a, B, window, st);
+    return D == 64 ? launch_prompt<__half, 64>(k_cache, v_cache, q, k, v, a, B, window, st)
+                   : launch_prompt<__half, 128>(k_cache, v_cache, q, k, v, a, B, window, st);
+}
+
+extern "C" int it_b200_attention_kvcache_prompt(int dtype, void *k_cache, void *v_cache, const void *q, const void *k,
+                                                const void *v, const void *position_id, int pos_flags, void *out, int B,
+                                                int Hq, int Hkv, int S, int S_max, int D, void *stream) {
+    return prompt_impl(dtype, k_cache, v_cache, q, k, v, position_id, pos_flags, out, B, Hq, Hkv, S, S_max, D, 0, stream);
+}
+
+extern "C" int it_b200_attention_kvcache_prompt_window(int dtype, void *k_cache, void *v_cache, const void *q, const void *k,
+                                                       const void *v, const void *position_id, int pos_flags, void *out, int B,
+                                                       int Hq, int Hkv, int S, int S_max, int D, int window, void *stream) {
+    ITB_CHECK(window >= 0, "AttentionKVCache prompt: window %d is negative", window);
+    return prompt_impl(dtype, k_cache, v_cache, q, k, v, position_id, pos_flags, out, B, Hq, Hkv, S, S_max, D, window, stream);
 }

@@ -65,6 +65,12 @@ def _require_head_width(h, dh: int):
         raise NotImplementedError(f"{type(h).__name__} does not execute {dh}-wide attention heads (the reference's are 128-wide)")
 
 
+def _require_window(h):
+    if not getattr(h, "sliding_window", False):
+        raise NotImplementedError(f"{type(h).__name__} has no sliding-window AttentionKVCache: it cannot run a config with "
+                                  "sliding_window (it would attend over every cache row)")
+
+
 def _require_rope_table(h, cfg):
     if not getattr(h, "rope_inv_freq", False):
         raise NotImplementedError(f"{type(h).__name__} has no RoPE inv_freq table: it cannot run rope_theta = {cfg.rope_theta}, "
@@ -119,6 +125,7 @@ class LlamaConfig:
     rope_theta: float = 10000.0  # RoPE base
     rope_scaling: dict | None = None  # None, or {"type": "llama3", factor, low_freq_factor, high_freq_factor,
                                       # original_max_position_embeddings} (see rope_inv_freq)
+    sliding_window: int | None = None  # every layer's query at position P attends over cache rows (P - W, P] only; None: all rows
 
     @property
     def n_kv(self) -> int:
@@ -145,6 +152,14 @@ class LlamaConfig:
                            rope_theta=500000.0, rope_scaling=dict(LLAMA31_ROPE_SCALING))
 
     @staticmethod
+    def mistral_7b_v01(batch=16, s_max=1024, dtype=BF16, layers=32, kv_fp8=False, int4_block=0):
+        """Mistral-7B-v0.1: 32 query heads over 8 KV heads of 128 (G = 4), ffn 14336, vocab 32000, RoPE base 10000 and a
+        sliding window of 4096 rows (HF's sliding_window).  The cache is indexed by absolute position: s_max covers the
+        longest position, not just the window."""
+        return LlamaConfig(layers=layers, d_model=4096, heads=32, kv_heads=8, head_dim=128, ffn=14336, vocab=32000,
+                           s_max=s_max, batch=batch, dtype=dtype, kv_fp8=kv_fp8, int4_block=int4_block, sliding_window=4096)
+
+    @staticmethod
     def tiny(dtype=BF16, layers=2, batch=4, kv_fp8=False):
         return LlamaConfig(layers=layers, d_model=256, heads=2, head_dim=128, ffn=512, vocab=1000, s_max=64,
                            batch=batch, dtype=dtype, kv_fp8=kv_fp8)
@@ -161,12 +176,14 @@ class LlamaConfig:
         return self.layers * per_layer + d + self.vocab * d + self.vocab * d  # + embedding table
 
     def algorithmic_bytes(self, pos: int, world: int = 1) -> int:
-        """SURVEY.md 8(d): weights read once + KV read/append + ~12 activation tensors per layer."""
+        """SURVEY.md 8(d): weights read once + KV read/append + ~12 activation tensors per layer.  With a sliding window W a
+        step reads min(pos + 1, W) cache rows per head instead of pos + 1."""
         e = 2 if self.dtype in (F16, BF16) else 4
         d, f, dkv = self.d_model, self.ffn, self.n_kv * self.head_dim
         proj = self.layers * ((2 * d * d + 2 * d * dkv + 3 * d * f) // world) + d * self.vocab
         norms = self.layers * 2 * d + d
-        kv = self.layers * 2 * self.batch * (self.n_kv // world) * self.head_dim * (pos + 2)
+        rows = pos + 2 if not self.sliding_window else min(pos + 1, self.sliding_window) + 1  # rows read + the appended one
+        kv = self.layers * 2 * self.batch * (self.n_kv // world) * self.head_dim * rows
         act = self.layers * 12 * self.batch * d
         kv_bytes = kv * e
         if self.kv_fp8:  # one byte per cache element + the 4-byte k / v scale of every KV head
@@ -216,6 +233,11 @@ def build_llama_decode(h, cfg: LlamaConfig, world: int = 1, rank: int = 0, seq: 
     rope_kw = {} if dh == 128 else {"dim_head": dh}  # 128-wide graphs make the reference's RoPE call
     if not cfg.rope_default:
         _require_rope_table(h, cfg)
+    if cfg.sliding_window is not None and cfg.sliding_window < 0:
+        raise ValueError(f"sliding_window = {cfg.sliding_window}: a window is at least 1 row (None: no window)")
+    if cfg.sliding_window:
+        _require_window(h)
+    win_kw = {"window": cfg.sliding_window} if cfg.sliding_window else {}  # (unwindowed: the call as before)
     g = LlamaGraph(cfg)
 
     def weight(name, shape, kind, shard=None):
@@ -285,7 +307,8 @@ def build_llama_decode(h, cfg: LlamaConfig, world: int = 1, rank: int = 0, seq: 
             t = h.reshape(t, None, [B, seq, n, dh])
             return h.transpose(t, None, [0, 2, 1, 3])  # [B,n,seq,dh]
 
-        attn = h.attentionKVCache(kc, vc, heads(q), heads(k, Hkv), heads(v, Hkv), g.position_ids, None, **kv_scales)
+        attn = h.attentionKVCache(kc, vc, heads(q), heads(k, Hkv), heads(v, Hkv), g.position_ids, None, **kv_scales,
+                                  **win_kw)
         a = h.reshape(h.transpose(attn, None, [0, 2, 1, 3]), None, [B, seq, dl])
         o = linear(a, p + "wo", (dl, d), ("row", d))
         if world > 1:

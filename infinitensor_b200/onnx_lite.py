@@ -571,8 +571,12 @@ class OnnxStub:
             else:
                 T[out0] = h.RoPE(I(0), I(1), None, **kw)
         elif op == "AttentionKVCache":  # optional inputs 6, 7 (extension): k_scale / v_scale of FP8 E4M3 caches
-            scales = {"k_scale": I(6), "v_scale": I(7)} if len(nd.inputs) > 6 else {}
-            T[out0] = h.attentionKVCache(I(0), I(1), I(2), I(3), I(4), I(5), None, **scales)
+            kw = {"k_scale": I(6), "v_scale": I(7)} if len(nd.inputs) > 6 else {}
+            if int(a.get("window", 0)):  # int attribute window (extension): sliding-window attention, absent = 0 = none
+                if not getattr(h, "sliding_window", False):
+                    raise NotImplementedError(f"AttentionKVCache {nd.name}: {type(h).__name__} has no sliding window")
+                kw["window"] = int(a["window"])
+            T[out0] = h.attentionKVCache(I(0), I(1), I(2), I(3), I(4), I(5), None, **kw)
         elif op in ("MaxPool", "AveragePool"):
             k = a["kernel_shape"]
             d, p, s = a.get("dilations", [1, 1]), list(a.get("pads", [0, 0, 0, 0])), a.get("strides", [1, 1])
@@ -784,12 +788,14 @@ class OnnxExporter:
         return self._emit("RoPE", [pos, x] + ([inv_freq] if inv_freq is not None else []),
                           self.inner.RoPE(pos.inner, x.inner, self._in(y), *extra, **kw), {"dim_head": extra[0]} if extra else None)
 
-    def attentionKVCache(self, kc, vc, q, k, v, pos, y, k_scale=None, v_scale=None):
-        # the FP8 caches' scales only when given: every 16-bit export stays as it was
+    def attentionKVCache(self, kc, vc, q, k, v, pos, y, k_scale=None, v_scale=None, window=0):
+        # the FP8 caches' scales and the window only when given: every other export stays as it was
         scales = [] if k_scale is None else [k_scale, v_scale]
-        r = self.inner.attentionKVCache(kc.inner, vc.inner, q.inner, k.inner, v.inner, pos.inner, self._in(y),
-                                        **({"k_scale": k_scale.inner, "v_scale": v_scale.inner} if scales else {}))
-        return self._emit("AttentionKVCache", [kc, vc, q, k, v, pos] + scales, r)
+        kw = {"k_scale": k_scale.inner, "v_scale": v_scale.inner} if scales else {}
+        if window:
+            kw["window"] = window
+        r = self.inner.attentionKVCache(kc.inner, vc.inner, q.inner, k.inner, v.inner, pos.inner, self._in(y), **kw)
+        return self._emit("AttentionKVCache", [kc, vc, q, k, v, pos] + scales, r, {"window": int(window)} if window else None)
 
     def _pool(self, op, fn, x, y, kh, kw, dh, dw, ph, pw, sh, sw, ceil):
         r = fn(x.inner, self._in(y), kh, kw, dh, dw, ph, pw, sh, sw, ceil)
