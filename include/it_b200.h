@@ -308,6 +308,8 @@ int it_b200_conv2d_nhwc(int dtype, const void *x, const void *w, void *y, int y_
 #define ITB_POS_IN_STEP 0x200 /* OR into pos_dtype: position_id / the RoPE positions / cache rows below the position may be written by a
                                  kernel of the SAME step (in-graph position arithmetic, a Concat of the past): nothing is read ahead of
                                  griddepcontrol.wait */
+#define ITB_POS_RING 0x400    /* OR into pos_flags: the caches are a rolling buffer (sliding-window launchers only; see
+                                 it_b200_attention_kvcache_window) */
 int64_t it_b200_attention_kvcache_workspace(int B, int H, int S_max, int D);
 int it_b200_attention_kvcache(int dtype, void *k_cache, void *v_cache, const void *q,
                               const void *k, const void *v, const void *position_id,
@@ -391,14 +393,23 @@ int it_b200_attention_kvcache_prompt(int dtype, void *k_cache, void *v_cache, co
 /* ---- Sliding-window attention (Mistral-7B-v0.1 and models trained like it).  window >= 1: the query at position P reads only
  *      cache rows j with P - window < j <= P, its own row included (transformers' `kv_idx > q_idx - sliding_window`; the
  *      original Mistral code keeps one row more: pass window + 1 for that).  Positions, clamping and the append are unchanged;
- *      the cache is still indexed by absolute position, so S_max must cover the longest position.  Rows below a query's window
+ *      without ITB_POS_RING the cache is indexed by absolute position, so S_max must cover the longest position.  Rows below a query's window
  *      never reach its output, even when they hold NaN.  window 0 is no window: the same kernels as the unwindowed calls.
  *      window < 0 is refused, before any launch.
  *   _window: every decode variant in one call.  k_scale / v_scale NULL: 16-bit or fp32 caches, non-NULL: FP8 E4M3 caches
  *      (it_b200_attention_kvcache_fp8); rope_pos NULL: no RoPE; inv_freq NULL: base 10000, else the table
  *      (it_b200_attention_kvcache_gqa_freq, freq_dtype / freq_len checked alike).  A windowed head streams only the rows
  *      [max(0, P - window + 1), P): min(P + 1, window) rows per step instead of P + 1.
- *   _prompt_window: it_b200_attention_kvcache_prompt, query i of batch row b reading rows (p_b + i - window, p_b + i]. ---- */
+ *   _prompt_window: it_b200_attention_kvcache_prompt, query i of batch row b reading rows (p_b + i - window, p_b + i].
+ *   Rolling cache (ITB_POS_RING in pos_flags, these two launchers only; Mistral's "rolling buffer cache"): the caches
+ *      [B, Hkv, S_max, D] are a ring, position P in row P mod S_max, so S_max bounds the window, not the context.  The
+ *      attention rule is the window's; the append writes row P mod S_max.  Positions are clamped to
+ *      [0, INT32_MAX - S_max] instead of S_max - 1 (S_max - S for a prompt), int64 ones before they are narrowed.  A ring
+ *      call is bit for bit the windowed call over a linear cache holding the same positions.  Refused before any launch:
+ *      window 0, S_max < window (the window and the row being appended must be distinct rows), S_max % 64 != 0 (a prompt
+ *      key tile never straddles the wrap), and a prompt chunk with S_max < window + S - 1 (its appends would overwrite
+ *      rows its own earlier queries read; split the prompt into chunks of at most S_max - window + 1 tokens).  Every
+ *      other AttentionKVCache launcher refuses the flag. ---- */
 int it_b200_attention_kvcache_window(int dtype, void *k_cache, void *v_cache, const void *k_scale, const void *v_scale,
                                      const void *q, const void *k, const void *v, const void *rope_pos, int rope_pos_dtype,
                                      const void *inv_freq, int freq_dtype, int64_t freq_len, int window, const void *position_id,

@@ -310,6 +310,7 @@ class GraphHandler:
     head_widths = (64, 128)  # decode attention / RoPE head widths (64: extension; the reference's are 128)
     rope_inv_freq = True  # RoPE takes the model's frequencies as an optional inv_freq input (extension)
     sliding_window = True  # AttentionKVCache takes a sliding window (extension)
+    rolling_cache = True  # a windowed AttentionKVCache's caches may be a ring (extension)
 
     def __init__(self, runtime: CudaRuntime):
         if not isinstance(runtime, CudaRuntime):
@@ -434,19 +435,24 @@ class GraphHandler:
         return self._op1("Concat", list(inputs), output, [dim])
 
     def attentionKVCache(self, input_k_cache, input_v_cache, input_q, input_k, input_v, position_id, output_matmul,
-                         per_row_positions=False, k_scale=None, v_scale=None, window=0):
+                         per_row_positions=False, k_scale=None, v_scale=None, window=0, rolling=False):
         """per_row_positions (extension, SURVEY 8(f-3)): batch row b attends up to / appends at position_id[b]; the default is
         the reference's rule -- element 0 for every row (attention_kvcache.cu:17).
         k_scale / v_scale (extension): the caches hold FP8 E4M3 codes (dtype 17), element value e4m3(code) * scale[KV head];
         both f32 [Hkv], given together, exactly when the caches are FP8.  One token per step, f16 / bf16 q / k / v.
         window (extension): sliding-window attention, the query at position P attends over cache rows (P - window, P] only
-        (HF's sliding_window); 0 = no window.  Decode and prompt steps, every cache type; a negative window is refused."""
+        (HF's sliding_window); 0 = no window.  Decode and prompt steps, every cache type; a negative window is refused.
+        rolling (extension, needs a window): the caches [B, Hkv, S_max, D] are a ring, position P in row P mod S_max, so S_max
+        bounds the window rather than the context (Mistral's rolling buffer cache).  S_max >= window, S_max % 64 == 0, and a
+        prompt chunk of S tokens needs S_max >= window + S - 1."""
         ins = [input_k_cache, input_v_cache, input_q, input_k, input_v, position_id]
         if (k_scale is None) != (v_scale is None):
             raise ValueError("attentionKVCache: k_scale and v_scale go together")
         if k_scale is not None:
             ins += [k_scale, v_scale]
         attrs = [int(bool(per_row_positions)), int(window)] if window else ([1] if per_row_positions else [])
+        if rolling:
+            attrs = [int(bool(per_row_positions)), int(window), 1]
         return self._op1("AttentionKVCache", ins, output_matmul, attrs)
 
     def RoPE(self, pos, input, output, dim_head=128, inv_freq=None):

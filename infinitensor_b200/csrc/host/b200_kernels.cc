@@ -560,6 +560,7 @@ static int attnPosFlags(const Operator &att, const Tensor &ropePos, const Tensor
     if (ropePos && ropePos->getSource() != nullptr) inStep = true;
     if (invFreq && invFreq->getSource() != nullptr) inStep = true;
     if (inStep) flags |= ITB_POS_IN_STEP;
+    if (as<AttentionKVCacheObj>(att)->getRolling()) flags |= ITB_POS_RING;  // (a windowed operator: the shape rule)
     return flags;
 }
 // RoPE(q), RoPE(k) folded into the decode attention kernel (the aliases between them are storage no-ops); the schedule folds

@@ -251,11 +251,12 @@ static Operator build_op(itb_graph *h, const string &name, const TensorVec &in, 
         need(2);
         return g->addOp<ConvObj>(in[0], in[1], o0, (int)I(0), (int)I(1), (int)I(2, 1), (int)I(3, 1), (int)I(4, 1),
                                  (int)I(5, 1));
-    case OpType::AttentionKVCache:  // iattr 0: per-row positions, 1: sliding window (both extensions)
+    case OpType::AttentionKVCache:  // iattr 0: per-row positions, 1: sliding window, 2: rolling cache (all extensions)
         need(6);
         IT_ASSERT(in.size() == 6 || in.size() == 8, "AttentionKVCache: 6 inputs, or 8 with an FP8 cache's k_scale / v_scale");
         return g->addOp<AttentionKVCacheObj>(in[0], in[1], in[2], in[3], in[4], in[5], o0, (bool)I(0, 0),
-                                             in.size() == 8 ? in[6] : nullptr, in.size() == 8 ? in[7] : nullptr, (int)I(1, 0));
+                                             in.size() == 8 ? in[6] : nullptr, in.size() == 8 ? in[7] : nullptr, (int)I(1, 0),
+                                             (bool)I(2, 0));
     case OpType::Softmax: need(1); return g->addOp<SoftmaxObj>(in[0], o0, (int)I(0, -1));
     case OpType::LayerNormalization:
         need(2);

@@ -136,11 +136,12 @@ static TensorVec attentionInputs(TensorVec v, Tensor kScale, Tensor vScale) {
 }
 AttentionKVCacheObj::AttentionKVCacheObj(GraphObj *graph, Tensor input_k_cache, Tensor input_v_cache,
                                          Tensor input_q, Tensor input_k, Tensor input_v, Tensor position_id,
-                                         Tensor output_matmul, bool perRowPositions, Tensor k_scale, Tensor v_scale, int window)
+                                         Tensor output_matmul, bool perRowPositions, Tensor k_scale, Tensor v_scale, int window,
+                                         bool rolling)
     : OperatorObj(OpType::AttentionKVCache,
                   attentionInputs({input_k_cache, input_v_cache, input_q, input_k, input_v, position_id}, k_scale, v_scale),
                   {output_matmul}),
-      perRowPositions(perRowPositions), window(window) {
+      perRowPositions(perRowPositions), window(window), rolling(rolling) {
     IT_ASSERT(checkValid(graph));
 }
 std::optional<vector<Shape>> AttentionKVCacheObj::inferShape(const TensorVec &ins) {
@@ -179,6 +180,16 @@ std::optional<vector<Shape>> AttentionKVCacheObj::inferShape(const TensorVec &in
         const int64_t np = (int64_t)ins[5]->size();
         IT_ASSERT(np == (int64_t)q[0] || np == (int64_t)q[0] * q[2],
                   "AttentionKVCache: a prompt chunk takes one position per batch row or one per token");
+    }
+    if (rolling) {  // a rolling cache (extension): position P in row P mod S_max
+        const std::string smax = std::to_string(c[2]), win = std::to_string(window);
+        IT_ASSERT(window >= 1, "AttentionKVCache: a rolling cache needs a window >= 1");
+        IT_ASSERT(c[2] >= window, "AttentionKVCache: a rolling cache of " + smax + " rows is shorter than the window of " + win);
+        IT_ASSERT(c[2] % 64 == 0, "AttentionKVCache: a rolling cache's length " + smax + " is not a multiple of 64");
+        IT_ASSERT(c[2] >= (int64_t)window + q[2] - 1,
+                  "AttentionKVCache: a chunk of " + std::to_string(q[2]) + " tokens needs a rolling cache of window + " +
+                      std::to_string(q[2] - 1) + " = " + std::to_string((int64_t)window + q[2] - 1) + " rows or more, not " +
+                      smax + " (split the prompt)");
     }
     return {{ins[2]->getDims()}};
 }

@@ -87,19 +87,24 @@ class ConvObj : public OperatorObj {
 class AttentionKVCacheObj : public OperatorObj {
     bool perRowPositions;  // extension (SURVEY 8(f-3)): row b attends up to position_id[b]; false = the reference's element-0 rule
     int window;            // extension: sliding window, query at position P reads rows (P - window, P]; 0 = no window
+    bool rolling;          // extension (needs a window): the caches are a ring, position P in row P mod S_max
 
   public:
     // k_scale / v_scale (extension): the caches hold FP8 E4M3 codes, element value e4m3(code) * scale[KV head]; f32 [Hkv]
     AttentionKVCacheObj(GraphObj *graph, Tensor input_k_cache, Tensor input_v_cache, Tensor input_q,
                         Tensor input_k, Tensor input_v, Tensor position_id, Tensor output_matmul,
-                        bool perRowPositions = false, Tensor k_scale = nullptr, Tensor v_scale = nullptr, int window = 0);
+                        bool perRowPositions = false, Tensor k_scale = nullptr, Tensor v_scale = nullptr, int window = 0,
+                        bool rolling = false);
     bool getPerRowPositions() const { return perRowPositions; }
     int getWindow() const { return window; }
+    bool getRolling() const { return rolling; }
     bool isFp8Cache() const { return inputs.size() == 8; }
-    // window 0 keeps the attribute vector (and with it perf records and capture keys) of an unwindowed operator
+    // window 0 keeps the attribute vector (and with it perf records and capture keys) of an unwindowed operator, and
+    // rolling false that of a windowed one
     vector<int> getOpAttrVector() const override {
         if (!window) return {(int)type.underlying(), (int)perRowPositions};
-        return {(int)type.underlying(), (int)perRowPositions, window};
+        if (!rolling) return {(int)type.underlying(), (int)perRowPositions, window};
+        return {(int)type.underlying(), (int)perRowPositions, window, 1};
     }
     std::optional<vector<Shape>> inferShape(const TensorVec &inputs) override;
     vector<DataType> inferDataType(const TensorVec &ins) const override { return {ins[2]->getDType()}; }

@@ -36,6 +36,30 @@ template <typename T, int D> struct RowCfg {
 template <int D> __host__ __device__ constexpr float attn_scale() { return D == 128 ? 0.08838834764831845f : 0.125f; }
 
 template <typename P> __device__ __forceinline__ int read_pos(const void *p, int i) { return (int)((const P *)p)[i]; }
+// a windowed body's position i: narrowed, then clamped to [0, Smax - 1] over a linear cache (the unwindowed rule); over a
+// ring (ITB_POS_RING) clamped to [0, ring_pos_max(Smax)] first, so that an int64 position is never wrapped by the narrowing
+__device__ __forceinline__ int win_pos(const void *position_id, int pos_dtype, int i, int Smax, bool ring) {
+    int64_t p = pos_dtype == ITB_I64 ? ((const int64_t *)position_id)[i] : (int64_t)read_pos<int32_t>(position_id, i);
+    if (!ring) p = (int)p;
+    return (int)min(max(p, (int64_t)0), (int64_t)(ring ? ring_pos_max(Smax) : Smax - 1));
+}
+// a windowed body's bulk copy of `rows` K and V rows from position `p0` of cache head `head` into a ring stage (K at dst, V
+// at dst + chunk_bytes), completing `bytes` = rows x D x sizeof(KT) on `bar` each.  Over a ring, a run of rows that crosses
+// the ring's end is two copies into consecutive addresses of the stage: both pieces are whole rows of D x sizeof(KT) >= 64
+// bytes, so they stay 16-byte aligned multiples of 16 bytes, and the stage's transaction count is unchanged
+template <typename KT, int D>
+__device__ __forceinline__ void win_chunk_load(unsigned char *dst, int chunk_bytes, const KT *kcache, const KT *vcache, int64_t head,
+                                               int Smax, int p0, int rows, bool ring, uint64_t *bar, uint64_t policy) {
+    const uint32_t bytes = (uint32_t)rows * D * (uint32_t)sizeof(KT);
+    const int r0 = cache_row(p0, Smax, ring);
+    const uint32_t b0 = (uint32_t)min(rows, Smax - r0) * D * (uint32_t)sizeof(KT);  // rows before the ring's end
+    const int64_t off = (head * Smax + r0) * D, wrap = head * Smax * D;
+    mbar_expect_tx(bar, 2 * bytes);
+    bulk_load_1d(dst, kcache + off, b0, bar, policy);
+    if (b0 < bytes) bulk_load_1d(dst + b0, kcache + wrap, bytes - b0, bar, policy);
+    bulk_load_1d(dst + chunk_bytes, vcache + off, b0, bar, policy);
+    if (b0 < bytes) bulk_load_1d(dst + chunk_bytes + b0, vcache + wrap, bytes - b0, bar, policy);
+}
 
 // ------------------------------------------------------------------------------------------------------------------
 // attn_stream_kernel: the production decode kernel.  Same arithmetic per cache row as attn_decode_kernel, but
@@ -164,6 +188,8 @@ __device__ __forceinline__ void
     // Units, offsets and the dealing count from lo, so a windowed head at p runs exactly as an unwindowed one at span(p)
     // over the cache rows from lo up
     auto span = [&](int p) { return WIN ? min(p, window - 1) : p; };
+    // (WIN) ITB_POS_RING: the caches are a ring, position p in row cache_row(p, Smax, rolling) = p mod Smax
+    const bool rolling = WIN && (pos_flags & ITB_POS_RING) != 0;
     if (threadIdx.x == 0) {
         for (int s = 0; s < AS_STAGES; ++s) {
             mbar_init(&full[s], 1);
@@ -172,9 +198,13 @@ __device__ __forceinline__ void
         fence_mbar_init();
     }
     for (int b = threadIdx.x; b < Bn; b += blockDim.x) {
-        int p = pos_dtype == ITB_I64 ? read_pos<int64_t>(position_id, per_row ? b : 0)
-                                     : read_pos<int32_t>(position_id, per_row ? b : 0);
-        s_pos[b] = min(max(p, 0), Smax - 1);
+        if constexpr (WIN) {
+            s_pos[b] = win_pos(position_id, pos_dtype, per_row ? b : 0, Smax, rolling);
+        } else {
+            int p = pos_dtype == ITB_I64 ? read_pos<int64_t>(position_id, per_row ? b : 0)
+                                         : read_pos<int32_t>(position_id, per_row ? b : 0);
+            s_pos[b] = min(max(p, 0), Smax - 1);
+        }
     }
     __syncthreads();
     if (threadIdx.x == 0) {
@@ -187,7 +217,8 @@ __device__ __forceinline__ void
     }
     __syncthreads();
     // Everything this step produced (q, k, v) is read by the consumers, after their wait; this kernel's own append
-    // touches row `pos` only, which the bulk loads never include.
+    // touches row `pos` only, which the bulk loads never include.  Over a ring that row, pos mod Smax, holds position
+    // pos - Smax or older, and Smax >= window (check_ring) puts that below the window, so no chunk includes it either.
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int64_t total = s_pre[Bn], G = min((int64_t)gridDim.x, total);
@@ -227,7 +258,13 @@ __device__ __forceinline__ void
             for (int it = 0; it < nunits; ++it) {
                 mbar_wait(&empty[st], ph ^ 1);
                 const int rows = min(CH, span(pos) - c * CH);
-                if (rows > 0) {
+                if constexpr (WIN) {
+                    if (rows > 0)
+                        win_chunk_load<KT, D>(ring + (size_t)st * 2 * CHUNK_BYTES, CHUNK_BYTES, kcache, vcache, bh, Smax,
+                                              pos - span(pos) + c * CH, rows, rolling, &full[st], policy);
+                    else
+                        mbar_arrive(&full[st]);
+                } else if (rows > 0) {
                     const uint32_t bytes = (uint32_t)rows * D * (uint32_t)sizeof(KT);
                     const int64_t off = ((int64_t)bh * Smax + (pos - span(pos)) + (int64_t)c * CH) * D;
                     mbar_expect_tx(&full[st], 2 * bytes);
@@ -398,13 +435,13 @@ __device__ __forceinline__ void
                 float vdec[EPL];
                 if constexpr (KV8<KT>) {
                     const uint4 vcodes = quantise_e4m3x16({ld16(vin + src), ld16(vin + src + VE)}, v_scale[bh % H]);
-                    *reinterpret_cast<uint4 *>(kcache + ((int64_t)bh * Smax + pos) * D + col) = kcodes;
-                    *reinterpret_cast<uint4 *>(vcache + ((int64_t)bh * Smax + pos) * D + col) = vcodes;
+                    *reinterpret_cast<uint4 *>(kcache + ((int64_t)bh * Smax + (WIN ? cache_row(pos, Smax, rolling) : pos)) * D + col) = kcodes;
+                    *reinterpret_cast<uint4 *>(vcache + ((int64_t)bh * Smax + (WIN ? cache_row(pos, Smax, rolling) : pos)) * D + col) = vcodes;
                     e4m3x16_to_f(vcodes, vdec);
                 } else {
                     vx = ld16(vin + src);
-                    st16(kcache + ((int64_t)bh * Smax + pos) * D + col, kx[0]);
-                    st16(vcache + ((int64_t)bh * Smax + pos) * D + col, vx);
+                    st16(kcache + ((int64_t)bh * Smax + (WIN ? cache_row(pos, Smax, rolling) : pos)) * D + col, kx[0]);
+                    st16(vcache + ((int64_t)bh * Smax + (WIN ? cache_row(pos, Smax, rolling) : pos)) * D + col, vx);
                 }
                 const float mx2 = fmaxf(m, d);
                 const float corr = expf(m - mx2), pnew = expf(d - mx2);
@@ -570,10 +607,16 @@ __device__ __forceinline__ void
     const int pos_dtype = pos_flags & 0xff;
     const bool per_row = (pos_flags & ITB_POS_PER_ROW) != 0;
     if (pos_flags & ITB_POS_IN_STEP) pdl_wait();  // (see attn_stream_kernel)
+    // (WIN) ITB_POS_RING as in attn_stream_body, the flag read where it is used: a named local for it changes how the
+    // unwindowed fp32 instantiations compile
     auto pos_of = [&](int b) {
-        const int p = pos_dtype == ITB_I64 ? read_pos<int64_t>(position_id, per_row ? b : 0)
-                                           : read_pos<int32_t>(position_id, per_row ? b : 0);
-        return min(max(p, 0), Smax - 1);
+        if constexpr (WIN) {
+            return win_pos(position_id, pos_dtype, per_row ? b : 0, Smax, (pos_flags & ITB_POS_RING) != 0);
+        } else {
+            const int p = pos_dtype == ITB_I64 ? read_pos<int64_t>(position_id, per_row ? b : 0)
+                                               : read_pos<int32_t>(position_id, per_row ? b : 0);
+            return min(max(p, 0), Smax - 1);
+        }
     };
     auto span = [&](int p) { return WIN ? min(p, window - 1) : p; };  // (see attn_stream_body)
     if (threadIdx.x == 0) {
@@ -639,11 +682,16 @@ __device__ __forceinline__ void
                 mbar_wait(&empty[st], ph ^ 1);
                 const int rows = min(CH, span(pos) - c * CH);
                 if (rows > 0) {
-                    const uint32_t bytes = (uint32_t)rows * D * (uint32_t)sizeof(KT);
-                    const int64_t off = ((int64_t)(bh / NQG) * Smax + (pos - span(pos)) + (int64_t)c * CH) * D;
-                    mbar_expect_tx(&full[st], 2 * bytes);
-                    bulk_load_1d(ring + (size_t)st * 2 * CHUNK_BYTES, kcache + off, bytes, &full[st], policy);
-                    bulk_load_1d(ring + (size_t)st * 2 * CHUNK_BYTES + CHUNK_BYTES, vcache + off, bytes, &full[st], policy);
+                    if constexpr (WIN) {
+                        win_chunk_load<KT, D>(ring + (size_t)st * 2 * CHUNK_BYTES, CHUNK_BYTES, kcache, vcache, bh / NQG, Smax,
+                                              pos - span(pos) + c * CH, rows, (pos_flags & ITB_POS_RING) != 0, &full[st], policy);
+                    } else {
+                        const uint32_t bytes = (uint32_t)rows * D * (uint32_t)sizeof(KT);
+                        const int64_t off = ((int64_t)(bh / NQG) * Smax + (pos - span(pos)) + (int64_t)c * CH) * D;
+                        mbar_expect_tx(&full[st], 2 * bytes);
+                        bulk_load_1d(ring + (size_t)st * 2 * CHUNK_BYTES, kcache + off, bytes, &full[st], policy);
+                        bulk_load_1d(ring + (size_t)st * 2 * CHUNK_BYTES + CHUNK_BYTES, vcache + off, bytes, &full[st], policy);
+                    }
                 } else {
                     mbar_arrive(&full[st]);
                 }
@@ -731,10 +779,10 @@ __device__ __forceinline__ void
                             const float *const scales[2] = {kv_scale...};
                             const uint2 codes = quantise_e4m3x8(x, scales[which][kv % Hkv]);
                             if (bh % NQG == 0)
-                                *reinterpret_cast<uint2 *>((which == 0 ? kcache : vcache) + (kv * Smax + pos) * D + col) = codes;
+                                *reinterpret_cast<uint2 *>((which == 0 ? kcache : vcache) + (kv * Smax + (WIN ? cache_row(pos, Smax, (pos_flags & ITB_POS_RING) != 0) : pos)) * D + col) = codes;
                             *reinterpret_cast<uint2 *>((which == 0 ? ks : vs) + nvalid * D + col) = codes;
                         } else {
-                            if (bh % NQG == 0) st16((which == 0 ? kcache : vcache) + (kv * Smax + pos) * D + col, x);
+                            if (bh % NQG == 0) st16((which == 0 ? kcache : vcache) + (kv * Smax + (WIN ? cache_row(pos, Smax, (pos_flags & ITB_POS_RING) != 0) : pos)) * D + col, x);
                             st16((which == 0 ? ks : vs) + nvalid * D + col, x);
                         }
                     }
@@ -1256,6 +1304,8 @@ static int attention_impl(int dtype, void *k_cache, void *v_cache, const void *q
     ITB_CHECK(D == 64 || D == 128, "AttentionKVCache: head dim %d is not supported (64 or 128)", D);
     ITB_CHECK(pos_dtype == ITB_I32 || pos_dtype == ITB_U32 || pos_dtype == ITB_I64,
               "AttentionKVCache: position dtype %d must be int32/uint32/int64", pos_dtype);
+    ITB_CHECK(window > 0 || !(pos_flags & ITB_POS_RING),
+              "AttentionKVCache: a rolling cache (ITB_POS_RING) needs a window: it_b200_attention_kvcache_window");
     ITB_CHECK(!rope_pos || rope_pos_dtype == ITB_I32 || rope_pos_dtype == ITB_U32 || rope_pos_dtype == ITB_I64,
               "AttentionKVCache: rope position dtype %d must be int32/uint32/int64", rope_pos_dtype);
     ITB_CHECK(aligned16(k_cache) && aligned16(v_cache) && aligned16(q) && aligned16(k) && aligned16(v),
@@ -1359,13 +1409,15 @@ extern "C" int it_b200_attention_kvcache_fp8_freq(int dtype, void *k_cache, void
 
 // Sliding-window decode over every cache type: k_scale / v_scale non-null, FP8 E4M3 codes; rope_pos non-null, RoPE folded in
 // (inv_freq non-null: the table's angles, else base 10000).  window >= 1: the query at position p reads rows (p - window, p];
-// window 0 runs the unwindowed kernels, as it_b200_attention_kvcache_gqa / _fp8 / _gqa_freq / _fp8_freq do
+// window 0 runs the unwindowed kernels, as it_b200_attention_kvcache_gqa / _fp8 / _gqa_freq / _fp8_freq do.  ITB_POS_RING:
+// the caches are a ring of S_max rows (check_ring)
 extern "C" int it_b200_attention_kvcache_window(int dtype, void *k_cache, void *v_cache, const void *k_scale, const void *v_scale,
                                                 const void *q, const void *k, const void *v, const void *rope_pos, int rope_pos_dtype,
                                                 const void *inv_freq, int freq_dtype, int64_t freq_len, int window,
                                                 const void *position_id, int pos_flags, void *out, int B, int Hq, int Hkv, int S_max,
                                                 int D, void *workspace, int64_t workspace_bytes, void *stream) {
     ITB_CHECK(window >= 0, "AttentionKVCache: window %d is negative", window);
+    if ((pos_flags & ITB_POS_RING) && check_ring("AttentionKVCache", window, S_max, 1)) return 1;
     ITB_CHECK(!k_scale == !v_scale, "AttentionKVCache(FP8 cache): k_scale and v_scale go together");
     if (inv_freq && check_inv_freq(k_scale ? "AttentionKVCache(FP8 cache)+RoPE" : "AttentionKVCache+RoPE", rope_pos, inv_freq,
                                    freq_dtype, freq_len, D))

@@ -411,28 +411,46 @@ struct PkArgs {
 };
 
 // p_b: element 0 of the positions, or (ITB_POS_PER_ROW) row b's first element at flat index b * stride; clamped to
-// [0, Smax - S] so that rows [p_b, p_b + S) lie in the cache
-__device__ __forceinline__ int prompt_start(const void *pos, int flags, int b, int S, int Smax) {
+// [0, Smax - S] so that rows [p_b, p_b + S) lie in the cache, or over a ring (ITB_POS_RING) to [0, ring_pos_max(Smax)]
+__device__ __forceinline__ int prompt_start(const void *pos, int flags, int b, int S, int Smax, bool ring = false) {
     const int stride = max(flags >> ITB_POS_ROW_STRIDE_SHIFT, 1);
     const int64_t i = (flags & ITB_POS_PER_ROW) ? (int64_t)b * stride : 0;
     const int64_t p = (flags & 0xff) == ITB_I64 ? ((const int64_t *)pos)[i] : (int64_t)((const int32_t *)pos)[i];
-    return (int)min(max(p, (int64_t)0), (int64_t)(Smax - S));
+    return (int)min(max(p, (int64_t)0), (int64_t)(ring ? ring_pos_max(Smax) : Smax - S));
 }
 
-// grid (ceil(S D / 8 / 256), B Hkv): one 16-byte chunk of k and of v per thread
-template <typename T>
-__global__ void __launch_bounds__(256) kvcache_append_kernel(T *__restrict__ kc, T *__restrict__ vc, const T *__restrict__ k,
-                                                             const T *__restrict__ v, const void *pos, int pos_flags, int Hkv,
-                                                             int S, int Smax, int D) {
+// grid (ceil(S D / 8 / 256), B Hkv): one 16-byte chunk of k and of v per thread.  RING: token i goes to row (p_b + i) mod Smax
+template <typename T, bool RING>
+__device__ __forceinline__ void append_body(T *__restrict__ kc, T *__restrict__ vc, const T *__restrict__ k, const T *__restrict__ v,
+                                            const void *pos, int pos_flags, int Hkv, int S, int Smax, int D) {
     pdl_trigger();
     pdl_wait();
     const int bh = blockIdx.y, b = bh / Hkv;
     const int64_t n = (int64_t)S * D / 8, c = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (c >= n) return;
-    const int p = prompt_start(pos, pos_flags, b, S, Smax);
-    const int64_t src = (int64_t)bh * S * D / 8 + c, dst = ((int64_t)bh * Smax + p) * D / 8 + c;
+    const int p = prompt_start(pos, pos_flags, b, S, Smax, RING);
+    const int64_t src = (int64_t)bh * S * D / 8 + c;
+    int64_t dst;
+    if constexpr (RING) {
+        const int i = (int)(c / (D / 8));  // the chunk's token
+        dst = ((int64_t)bh * Smax + cache_row(p + i, Smax, true)) * D / 8 + c % (D / 8);
+    } else {
+        dst = ((int64_t)bh * Smax + p) * D / 8 + c;
+    }
     reinterpret_cast<uint4 *>(kc)[dst] = reinterpret_cast<const uint4 *>(k)[src];
     reinterpret_cast<uint4 *>(vc)[dst] = reinterpret_cast<const uint4 *>(v)[src];
+}
+template <typename T>
+__global__ void __launch_bounds__(256) kvcache_append_kernel(T *__restrict__ kc, T *__restrict__ vc, const T *__restrict__ k,
+                                                             const T *__restrict__ v, const void *pos, int pos_flags, int Hkv,
+                                                             int S, int Smax, int D) {
+    append_body<T, false>(kc, vc, k, v, pos, pos_flags, Hkv, S, Smax, D);  // (pdl_trigger / pdl_wait inside)
+}
+template <typename T>
+__global__ void __launch_bounds__(256) kvcache_append_ring_kernel(T *__restrict__ kc, T *__restrict__ vc, const T *__restrict__ k,
+                                                                  const T *__restrict__ v, const void *pos, int pos_flags, int Hkv,
+                                                                  int S, int Smax, int D) {
+    append_body<T, true>(kc, vc, k, v, pos, pos_flags, Hkv, S, Smax, D);  // (pdl_trigger / pdl_wait inside)
 }
 
 // WIN (window >= 1): query i attends over rows (p_b + i - window, p_b + i] only.  Key tiles wholly below the tile's first query's
@@ -468,7 +486,12 @@ __device__ __forceinline__ void prompt_body(const CUtensorMap &mapQ, const CUten
     __syncthreads();
     pdl_wait();  // q / k / v and every cache row >= p_b are written in this step (the append launch)
 
-    const int p = prompt_start(a.pos, a.pos_flags, b, a.S, a.Smax);
+    // (WIN) ITB_POS_RING: the caches are a ring, key tile t at row cache_row(64 t), one TMA box as Smax % 64 == 0.  Every
+    // mask and limit below stays in positions.  Smax >= window + S - 1 (check_ring) keeps the positions the tile's queries
+    // read in distinct rows; the first tile's rows below lo0 and the last tile's rows past p + S - 1 may hold other
+    // positions (the chunk's own appends among them) and are made harmless like any rows outside the windows
+    const bool ring = WIN && (a.pos_flags & ITB_POS_RING) != 0;
+    const int p = prompt_start(a.pos, a.pos_flags, b, a.S, a.Smax, ring);
     const int last = p + min(i0 + PK_BQ - 1, a.S - 1);  // the tile's last query attends over rows 0 .. last
     const int nkt = last / PK_BK + 1;
     const int lo0 = WIN ? max(p + i0 - window + 1, 0) : 0;  // the first row of the tile's first query's window
@@ -480,8 +503,8 @@ __device__ __forceinline__ void prompt_body(const CUtensorMap &mapQ, const CUten
         mbar_expect_tx(&bar_kv[sg], 2 * TILE_BYTES);
 #pragma unroll
         for (int g = 0; g < DG; ++g) {
-            tma_load_3d(ks + g * (PK_BK * 128), &mapK, &bar_kv[sg], g * 64, t * PK_BK, kvh, pol);
-            tma_load_3d(vs + g * (PK_BK * 128), &mapV, &bar_kv[sg], g * 64, t * PK_BK, kvh, pol);
+            tma_load_3d(ks + g * (PK_BK * 128), &mapK, &bar_kv[sg], g * 64, cache_row(t * PK_BK, a.Smax, ring), kvh, pol);
+            tma_load_3d(vs + g * (PK_BK * 128), &mapV, &bar_kv[sg], g * 64, cache_row(t * PK_BK, a.Smax, ring), kvh, pol);
         }
     };
     if (threadIdx.x == 0) {
@@ -648,7 +671,8 @@ template <typename T, int D>
 static int launch_prompt(void *kc, void *vc, const void *q, const void *k, const void *v, const PkArgs &a, int B, int window,
                          cudaStream_t st) {
     const int64_t chunks = (int64_t)a.S * D / 8;
-    if (launch("AttentionKVCache prompt: append", kvcache_append_kernel<T>,
+    if (launch("AttentionKVCache prompt: append",
+               (a.pos_flags & ITB_POS_RING) ? kvcache_append_ring_kernel<T> : kvcache_append_kernel<T>,
                {dim3((unsigned)((chunks + 255) / 256), B * a.Hkv), dim3(256), 0, st}, (T *)kc, (T *)vc, (const T *)k, (const T *)v,
                a.pos, a.pos_flags, a.Hkv, a.S, a.Smax, D))
         return 1;
@@ -753,6 +777,8 @@ static int prompt_impl(int dtype, void *k_cache, void *v_cache, const void *q, c
     const int pos_dtype = pos_flags & 0xff;
     ITB_CHECK(pos_dtype == ITB_I32 || pos_dtype == ITB_U32 || pos_dtype == ITB_I64,
               "AttentionKVCache prompt: position dtype %d must be int32/uint32/int64", pos_dtype);
+    ITB_CHECK(window > 0 || !(pos_flags & ITB_POS_RING),
+              "AttentionKVCache prompt: a rolling cache (ITB_POS_RING) needs a window: it_b200_attention_kvcache_prompt_window");
     ITB_CHECK(B >= 0 && Hq >= 0 && S >= 1 && S <= S_max, "AttentionKVCache prompt: %d tokens do not fit a cache of %d rows", S, S_max);
     ITB_CHECK(Hkv > 0 && Hq % Hkv == 0, "AttentionKVCache prompt: %d query heads are not a multiple of %d KV heads", Hq, Hkv);
     ITB_CHECK((int64_t)B * Hq <= 65535 && (int64_t)B * Hkv <= 65535, "AttentionKVCache prompt: batch x heads beyond the grid limit");
@@ -786,5 +812,6 @@ extern "C" int it_b200_attention_kvcache_prompt_window(int dtype, void *k_cache,
                                                        const void *v, const void *position_id, int pos_flags, void *out, int B,
                                                        int Hq, int Hkv, int S, int S_max, int D, int window, void *stream) {
     ITB_CHECK(window >= 0, "AttentionKVCache prompt: window %d is negative", window);
+    if ((pos_flags & ITB_POS_RING) && check_ring("AttentionKVCache prompt", window, S_max, S)) return 1;
     return prompt_impl(dtype, k_cache, v_cache, q, k, v, position_id, pos_flags, out, B, Hq, Hkv, S, S_max, D, window, stream);
 }

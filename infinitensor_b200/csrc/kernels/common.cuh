@@ -166,6 +166,22 @@ __device__ __forceinline__ uint32_t f32x2_to_e4m3x2(float lo, float hi) {
 
 inline bool aligned16(const void *p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
 
+// ---- rolling KV cache (ITB_POS_RING): the one place that maps a position to its cache row ----------------------------
+// A ring of Smax rows holds position p in row p mod Smax; a linear cache, in row p.  Ring positions are clamped to
+// [0, ring_pos_max(Smax)], so that every position a step forms (below p + Smax) stays inside int
+__host__ __device__ constexpr int ring_pos_max(int Smax) { return 0x7fffffff - Smax; }
+__device__ __forceinline__ int cache_row(int p, int Smax, bool ring) { return ring ? p % Smax : p; }
+// the ring's shape rule, before any launch (S: tokens per step): 0, or 1 with the error set
+inline int check_ring(const char *what, int window, int Smax, int S) {
+    ITB_CHECK(window >= 1, "%s: a rolling cache (ITB_POS_RING) needs a window >= 1", what);
+    ITB_CHECK(Smax >= window, "%s: a rolling cache of %d rows is shorter than the window of %d", what, Smax, window);
+    ITB_CHECK(Smax % 64 == 0, "%s: a rolling cache's length %d is not a multiple of 64", what, Smax);
+    ITB_CHECK(S <= 1 || Smax >= (int64_t)window + S - 1,
+              "%s: a chunk of %d tokens needs a rolling cache of window + %d = %lld rows or more, not %d (split the prompt)", what,
+              S, S - 1, (long long)window + S - 1, Smax);
+    return 0;
+}
+
 // ---- reductions -----------------------------------------------------------------------------
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll

@@ -71,6 +71,12 @@ def _require_window(h):
                                   "sliding_window (it would attend over every cache row)")
 
 
+def _require_ring(h):
+    if not getattr(h, "rolling_cache", False):
+        raise NotImplementedError(f"{type(h).__name__} has no rolling KV cache: it cannot run a config with rolling_cache "
+                                  "(it would index the cache by absolute position)")
+
+
 def _require_rope_table(h, cfg):
     if not getattr(h, "rope_inv_freq", False):
         raise NotImplementedError(f"{type(h).__name__} has no RoPE inv_freq table: it cannot run rope_theta = {cfg.rope_theta}, "
@@ -126,6 +132,7 @@ class LlamaConfig:
     rope_scaling: dict | None = None  # None, or {"type": "llama3", factor, low_freq_factor, high_freq_factor,
                                       # original_max_position_embeddings} (see rope_inv_freq)
     sliding_window: int | None = None  # every layer's query at position P attends over cache rows (P - W, P] only; None: all rows
+    rolling_cache: bool = False  # (with a window) the caches are a ring of s_max rows, position P in row P mod s_max
 
     @property
     def n_kv(self) -> int:
@@ -152,12 +159,15 @@ class LlamaConfig:
                            rope_theta=500000.0, rope_scaling=dict(LLAMA31_ROPE_SCALING))
 
     @staticmethod
-    def mistral_7b_v01(batch=16, s_max=1024, dtype=BF16, layers=32, kv_fp8=False, int4_block=0):
+    def mistral_7b_v01(batch=16, s_max=1024, dtype=BF16, layers=32, kv_fp8=False, int4_block=0, rolling_cache=False):
         """Mistral-7B-v0.1: 32 query heads over 8 KV heads of 128 (G = 4), ffn 14336, vocab 32000, RoPE base 10000 and a
-        sliding window of 4096 rows (HF's sliding_window).  The cache is indexed by absolute position: s_max covers the
-        longest position, not just the window."""
+        sliding window of 4096 rows (HF's sliding_window).  By default the cache is indexed by absolute position: s_max
+        covers the longest position, not just the window.  rolling_cache=True makes it a ring of s_max rows (Mistral's
+        rolling buffer cache): s_max >= 4096 and a multiple of 64, and prompt chunks of up to s_max - 4095 tokens, so
+        s_max=4608 for 512-token chunks; decode then goes on past s_max."""
         return LlamaConfig(layers=layers, d_model=4096, heads=32, kv_heads=8, head_dim=128, ffn=14336, vocab=32000,
-                           s_max=s_max, batch=batch, dtype=dtype, kv_fp8=kv_fp8, int4_block=int4_block, sliding_window=4096)
+                           s_max=s_max, batch=batch, dtype=dtype, kv_fp8=kv_fp8, int4_block=int4_block, sliding_window=4096,
+                           rolling_cache=rolling_cache)
 
     @staticmethod
     def tiny(dtype=BF16, layers=2, batch=4, kv_fp8=False):
@@ -238,6 +248,16 @@ def build_llama_decode(h, cfg: LlamaConfig, world: int = 1, rank: int = 0, seq: 
     if cfg.sliding_window:
         _require_window(h)
     win_kw = {"window": cfg.sliding_window} if cfg.sliding_window else {}  # (unwindowed: the call as before)
+    if cfg.rolling_cache:
+        W = cfg.sliding_window
+        if not W:
+            raise ValueError("rolling_cache needs a sliding_window: a ring holds the window's rows")
+        need = W + seq - 1
+        if cfg.s_max < need or cfg.s_max % 64:
+            raise ValueError(f"rolling_cache: s_max = {cfg.s_max}, but a ring for window {W} and {seq}-token steps needs "
+                             f"s_max >= window + seq - 1 = {need} and a multiple of 64 (e.g. {-(-need // 64) * 64})")
+        _require_ring(h)
+        win_kw["rolling"] = True
     g = LlamaGraph(cfg)
 
     def weight(name, shape, kind, shard=None):

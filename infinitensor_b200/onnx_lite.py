@@ -576,6 +576,10 @@ class OnnxStub:
                 if not getattr(h, "sliding_window", False):
                     raise NotImplementedError(f"AttentionKVCache {nd.name}: {type(h).__name__} has no sliding window")
                 kw["window"] = int(a["window"])
+            if int(a.get("rolling", 0)):  # int attribute rolling (extension): the caches are a ring, absent = 0 = linear
+                if not getattr(h, "rolling_cache", False):
+                    raise NotImplementedError(f"AttentionKVCache {nd.name}: {type(h).__name__} has no rolling KV cache")
+                kw["rolling"] = True
             T[out0] = h.attentionKVCache(I(0), I(1), I(2), I(3), I(4), I(5), None, **kw)
         elif op in ("MaxPool", "AveragePool"):
             k = a["kernel_shape"]
@@ -788,14 +792,20 @@ class OnnxExporter:
         return self._emit("RoPE", [pos, x] + ([inv_freq] if inv_freq is not None else []),
                           self.inner.RoPE(pos.inner, x.inner, self._in(y), *extra, **kw), {"dim_head": extra[0]} if extra else None)
 
-    def attentionKVCache(self, kc, vc, q, k, v, pos, y, k_scale=None, v_scale=None, window=0):
-        # the FP8 caches' scales and the window only when given: every other export stays as it was
+    def attentionKVCache(self, kc, vc, q, k, v, pos, y, k_scale=None, v_scale=None, window=0, rolling=False):
+        # the FP8 caches' scales, the window and the ring only when given: every other export stays as it was
         scales = [] if k_scale is None else [k_scale, v_scale]
         kw = {"k_scale": k_scale.inner, "v_scale": v_scale.inner} if scales else {}
+        attrs = {}
         if window:
-            kw["window"] = window
+            kw["window"] = attrs["window"] = int(window)
+        if rolling:
+            if not getattr(self.inner, "rolling_cache", False):
+                raise NotImplementedError(f"AttentionKVCache: {type(self.inner).__name__} has no rolling KV cache")
+            kw["rolling"] = True
+            attrs["rolling"] = 1
         r = self.inner.attentionKVCache(kc.inner, vc.inner, q.inner, k.inner, v.inner, pos.inner, self._in(y), **kw)
-        return self._emit("AttentionKVCache", [kc, vc, q, k, v, pos] + scales, r, {"window": int(window)} if window else None)
+        return self._emit("AttentionKVCache", [kc, vc, q, k, v, pos] + scales, r, attrs or None)
 
     def _pool(self, op, fn, x, y, kh, kw, dh, dw, ph, pw, sh, sw, ceil):
         r = fn(x.inner, self._in(y), kh, kw, dh, dw, ph, pw, sh, sw, ceil)
